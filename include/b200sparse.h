@@ -72,7 +72,8 @@ int64_t     b2s_ws_bytes(void);
  *       syncs the stream once (the reference's partition tasks also block, fast_image_range.cu:27-54).
  *   b2s_spmv_plan_destroy: frees the host handle (never the device buffer).
  *   b2s_spmv_plan_info  : out[0]=tile config id, out[1]=bit0 row-group kernel, bit1 uniform-row path, bit2 scattered, bit3 short-row
- *                         (one lane per row) path, bit4 TMA tile kind, bit5 packed structure, out[2]=tiles,
+ *                         (one lane per row) path, bit4 TMA tile kind, bit5 packed structure, bit6 coded values,
+ *                         bits 8..12 distinct values of a coded plan, out[2]=tiles,
  *                         out[3]=1000*lines-per-warp statistic. */
 int64_t     b2s_spmv_plan_tiles(int vt, int64_t nrows, int64_t nnz);
 int64_t     b2s_spmv_plan_bytes(int vt, int64_t nrows, int64_t nnz);
@@ -96,10 +97,20 @@ int         b2s_spmv_plan_info(const void* plan, int64_t* out4_host);
  *   b2s_spmv_plan_pack      : fills it from the indptr / indices the plan was created for.  The buffer is caller-owned
  *                             like the plan buffer and must outlive every launch with the plan; an edit of indptr /
  *                             indices afterwards needs a new plan;
- *   b2s_spmv_plan_set_packed: 0 = launches read indptr / indices again, 1 = the packed form (tests / tools). */
+ *   b2s_spmv_plan_pack_coded: the same, and when `vals` holds at most 16 distinct bit patterns (-0.0 / +0.0 and NaN
+ *                             payloads count apart) and every tile's column window leaves vb = ceil(log2(distinct))
+ *                             spare bits in its uint16 words, each word also carries the index of its value in a
+ *                             sorted dictionary kept in the buffer (CSR-VI-style value indices): launches with this
+ *                             `vals` pointer then stream no values at all, launches with another `vals` pointer stream
+ *                             theirs.  An edit of vals afterwards (even in place) needs a new plan; otherwise it packs
+ *                             exactly as b2s_spmv_plan_pack;
+ *   b2s_spmv_plan_set_packed: 0 = launches read indptr / indices again, 1 = the packed form with streamed values,
+ *                             2 = the packed form with coded values (tests / tools). */
 int64_t     b2s_spmv_plan_pack_bytes(const void* plan);
 int         b2s_spmv_plan_pack(void* plan, const void* indptr, const void* indices, void* pack_buf_dev, void* stream);
-int         b2s_spmv_plan_set_packed(void* plan, int on);
+int         b2s_spmv_plan_pack_coded(void* plan, const void* indptr, const void* indices, const void* vals,
+                                     void* pack_buf_dev, void* stream);
+int         b2s_spmv_plan_set_packed(void* plan, int mode);
 
 /* y = A x  (alpha=1, beta=0 as spmv.cu:79-80).  `plan` may be NULL: then a plan-free
  * row-per-lane-group kernel is used (slower on short rows).  `plan` is the HOST handle

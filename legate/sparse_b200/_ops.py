@@ -35,7 +35,9 @@ class SpmvPlan:
     def __init__(self, handle: int, buf: torch.Tensor, pack_buf: torch.Tensor | None = None):
         self.handle = handle
         self.buf = buf
-        self.pack_buf = pack_buf   # the packed structure (b2s_spmv_plan_pack), read by every launch with this plan
+        # the packed structure (b2s_spmv_plan_pack / _pack_coded), read by every launch with this plan: it lives as long
+        # as the plan, and is never rewritten (a captured launch may still read it)
+        self.pack_buf = pack_buf
         self._info()
 
     def _info(self):
@@ -43,6 +45,7 @@ class SpmvPlan:
         _lib.check(L.b2s_spmv_plan_info(self.handle, out), "b2s_spmv_plan_info")
         self.config, self.rowgroup, self.uniform, self.scattered = int(out[0]), bool(out[1] & 1), bool(out[1] & 2), bool(out[1] & 4)
         self.short_rows, self.tma, self.packed = bool(out[1] & 8), bool(out[1] & 16), bool(out[1] & 32)
+        self.coded, self.ndict = bool(out[1] & 64), int(out[1] >> 8) & 31
         self.tiles, self.lines_per_warp = int(out[2]), out[3] / 1000.0
 
     @property
@@ -65,9 +68,10 @@ class SpmvPlan:
         _lib.check(L.b2s_spmv_plan_set_flavor(self.handle, int(flavor)), "b2s_spmv_plan_set_flavor")
         self._info()
 
-    def set_packed(self, on: bool):
-        """tools / tests: stream the packed structure (the plan must have been packed) or the CSR arrays."""
-        _lib.check(L.b2s_spmv_plan_set_packed(self.handle, int(bool(on))), "b2s_spmv_plan_set_packed")
+    def set_packed(self, mode):
+        """tools / tests: 0 / False = stream the CSR arrays, 1 / True = the packed structure and the values, 2 = the
+        packed structure with coded values (the plan must have been packed / coded)."""
+        _lib.check(L.b2s_spmv_plan_set_packed(self.handle, int(mode)), "b2s_spmv_plan_set_packed")
         self._info()
 
     @property
@@ -78,6 +82,8 @@ class SpmvPlan:
         fl = "short-rows(one lane per row)" if self.short_rows else ("uniform-rows" if self.uniform else "generic")
         if self.packed:
             fl += ", packed u16 columns/row offsets"
+        if self.coded:
+            fl += f", coded values ({self.ndict} distinct)"
         return f"b2s::spmv_{'tma' if self.tma else 'tile'}_kernel cfg {self.config} [{fl}]"
 
     def __del__(self):
@@ -97,7 +103,8 @@ def spmv_plan(indptr: torch.Tensor, indices: torch.Tensor, shape, nnz: int, vdty
     """Build the SpMV plan for a CSR structure (tile boundaries + kernel choice).  `tma_only`: the plan must use the
     TMA tile kernel (needed by spmv_add / spmv_fused).  When the library reports that the structure qualifies (short
     rows, every tile's columns within 65536 of each other) the plan is packed: its launches stream uint16 columns and
-    row offsets instead of `indices` / `indptr`, so the plan is only valid while those arrays are unchanged."""
+    row offsets instead of `indices` / `indptr`, so the plan is only valid while those arrays are unchanged.  See
+    spmv_plan_code for coding the values as well."""
     _chk_dev(indptr, indices)
     vt = vt_code(vdtype)
     nrows, ncols = shape
@@ -116,7 +123,25 @@ def spmv_plan(indptr: torch.Tensor, indices: torch.Tensor, shape, nnz: int, vdty
         if rc != _lib.OK:
             L.b2s_spmv_plan_destroy(handle)
             _lib.check(rc, "b2s_spmv_plan_pack")
-    return SpmvPlan(handle, buf, pack_buf)
+    plan = SpmvPlan(handle, buf, pack_buf)
+    plan.nnz = nnz
+    return plan
+
+
+def spmv_plan_code(plan: SpmvPlan, indptr: torch.Tensor, indices: torch.Tensor, data: torch.Tensor) -> SpmvPlan:
+    """Code the values of a packed plan that no launch has used yet: when `data` holds at most 16 distinct values (bit
+    patterns) and every tile's column window leaves room for their codes in the uint16 column words, the pack buffer
+    is rewritten with the codes, and launches with this `data` stream no values at all -- so the plan is then also only
+    valid while `data` is unchanged.  Otherwise the plan stays packed with streamed values.  A plan without a pack
+    buffer is returned as it is."""
+    if getattr(plan, "pack_buf", None) is None:
+        return plan
+    _chk_dev(data)
+    assert data.is_contiguous() and data.shape[0] == plan.nnz
+    _lib.check(L.b2s_spmv_plan_pack_coded(plan.handle, ptr(indptr), ptr(indices), ptr(data), ptr(plan.pack_buf),
+                                          _stream()), "b2s_spmv_plan_pack_coded")
+    plan._info()
+    return plan
 
 
 def spmv(indptr, indices, data, x, y, shape, plan=None):

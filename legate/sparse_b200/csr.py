@@ -275,12 +275,17 @@ class csr_array:
 
         tma_only = bool(tma_only or getattr(self, "_plan_tma_only", False))
         self._plan_tma_only = tma_only
-        # the versions: a packed plan holds its own copy of the structure, so an in-place edit of indices / indptr
-        # (same pointers) must build a new plan
+        # the versions: a packed plan holds its own copy of the structure, and a coded one of the values, so an
+        # in-place edit of indices / indptr / data (same pointers) must build a new plan -- a new one, never a rewrite
+        # of the old pack buffer, which a captured graph may still read
         key = (self._indptr.data_ptr(), self._indptr._version, self._indices.data_ptr(), self._indices._version,
+               self._data.data_ptr(), self._data._version,
                int(_lib.lib.b2s_spmv_get_config()), self.dtype.itemsize, self.nnz, tma_only)
         if self._plan is None or self._plan_key != key:
-            self._plan = _ops.spmv_plan(self._indptr, self._indices, self.shape, self.nnz, self.dtype, tma_only=tma_only)
+            plan = _ops.spmv_plan(self._indptr, self._indices, self.shape, self.nnz, self.dtype, tma_only=tma_only)
+            if self._data.is_contiguous():
+                plan = _ops.spmv_plan_code(plan, self._indptr, self._indices, self._data)
+            self._plan = plan
             self._plan_key = key
         return self._plan
 

@@ -4,8 +4,10 @@
 // Replaces CSRSpMVRowSplit::gpu_variant (reference src/sparse/array/csr/spmv.cu:24-123, a cusparseSpMV call) and
 // the partition helpers behind it (sparse/partition.py:56-208, src/sparse/partition/*.cu).
 #include "spmv_common.cuh"
+#include <algorithm>
 #include <atomic>
 #include <stdlib.h>
+#include <vector>
 
 namespace b2s {
 
@@ -141,15 +143,24 @@ spmv_col_window_kernel(const I* __restrict__ indices, const long long* __restric
   }
 }
 
-// Packing (see PackedTiles in spmv_common.cuh), one warp per tile.  WRITE = false: counts in *bad the tiles the packed
-// kernel cannot take -- a row-shape code other than short rows, or nonzeros more than 65535 columns apart; WRITE =
-// true: stores the tile's smallest column and its uint16 column and row-offset slices.  Tiles without rows are skipped
-// by the SpMV kernel and here.
+// Value dictionary of a packed plan (b2s_spmv_plan_pack_coded): the sorted distinct bit patterns of `vals` when there
+// are at most kMaxDict of them.  Bit patterns, not values, so -0.0 / +0.0 and NaN payloads stay apart.
+struct DictBits {
+  unsigned long long v[kMaxDict];
+  int n;
+};
+
+// Packing (see PackedTiles in spmv_common.cuh), one warp per tile.  WRITE = false: counts in stat[0] the tiles the
+// packed kernel cannot take -- a row-shape code other than short rows, or nonzeros more than 65535 columns apart -- and
+// raises stat[1] to the widest window (largest minus smallest column) of a tile; WRITE = true: stores the tile's
+// smallest column and its uint16 column and row-offset slices.  With coded values (vbytes = sizeof V, else 0) a column
+// word is (column - base) << vb | the index of the value's bit pattern in `dict`.  Tiles without rows are skipped by the
+// SpMV kernel and here.
 template <typename I, typename P, bool WRITE>
 __global__ void __launch_bounds__(256)
 spmv_pack_kernel(const P* __restrict__ indptr, const I* __restrict__ indices, const PlanEntry* __restrict__ plan,
                  int64_t ntiles, uint16_t* __restrict__ cols, uint16_t* __restrict__ rows, long long* __restrict__ base,
-                 unsigned long long* __restrict__ bad) {
+                 unsigned long long* __restrict__ stat, const void* __restrict__ vals, int vbytes, int vb, DictBits dict) {
   const int lane = threadIdx.x & 31;
   const int64_t t = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   if (t >= ntiles) return;
@@ -172,12 +183,23 @@ spmv_pack_kernel(const P* __restrict__ indptr, const I* __restrict__ indices, co
   const bool empty = k1 == k0;
   if (!WRITE) {
     const bool ok = e0.pad != 0 && e0.pad <= kShortRowMax && (empty || mx - mn <= 65535);
-    if (lane == 0 && !ok) atomicAdd(bad, 1ull);
+    if (lane == 0 && !ok) atomicAdd(stat, 1ull);
+    if (lane == 0 && !empty) atomicMax(stat + 1, (unsigned long long)(mx - mn));
     return;
   }
   const long long cb = empty ? 0 : mn;
   uint16_t* tc = cols + kPackColGap * t;
-  for (long long k = k0 + lane; k < k1; k += 32) tc[k] = (uint16_t)((long long)indices[k] - cb);
+  for (long long k = k0 + lane; k < k1; k += 32) {
+    unsigned w = (unsigned)((long long)indices[k] - cb);
+    if (vbytes) {
+      const unsigned long long bits = vbytes == 8 ? reinterpret_cast<const unsigned long long*>(vals)[k]
+                                                  : (unsigned long long)reinterpret_cast<const unsigned*>(vals)[k];
+      unsigned code = 0;
+      for (int i = 1; i < dict.n; i++) code = dict.v[i] == bits ? (unsigned)i : code;
+      w = (w << vb) | code;
+    }
+    tc[k] = (uint16_t)w;
+  }
   uint16_t* tr = rows + e0.row + kPackRowGap * t;
   const long long kb = k0 & ~3LL;
   for (int j = lane; j <= nr; j += 32) tr[j] = (uint16_t)((long long)indptr[e0.row + j] - kb);
@@ -186,25 +208,91 @@ spmv_pack_kernel(const P* __restrict__ indptr, const I* __restrict__ indices, co
 
 template <bool WRITE>
 static int launch_pack(int it, int pt, const void* indptr, const void* indices, const PlanEntry* plan, int64_t ntiles,
-                       PackedTiles pk, unsigned long long* bad, cudaStream_t st) {
+                       PackedTiles pk, unsigned long long* stat, const void* vals, int vbytes, const DictBits& dict,
+                       cudaStream_t st) {
   const unsigned grid = (unsigned)((ntiles * 32 + 255) / 256);
   uint16_t* c = const_cast<uint16_t*>(pk.cols);
   uint16_t* r = const_cast<uint16_t*>(pk.rows);
   long long* b = const_cast<long long*>(pk.base);
+  const int vb = pk.vb;
   if (it == B2S_I32 && pt == B2S_I32)
-    spmv_pack_kernel<int32_t, int32_t, WRITE><<<grid, 256, 0, st>>>((const int32_t*)indptr, (const int32_t*)indices, plan, ntiles, c, r, b, bad);
+    spmv_pack_kernel<int32_t, int32_t, WRITE><<<grid, 256, 0, st>>>((const int32_t*)indptr, (const int32_t*)indices, plan, ntiles, c, r, b, stat, vals, vbytes, vb, dict);
   else if (it == B2S_I32)
-    spmv_pack_kernel<int32_t, int64_t, WRITE><<<grid, 256, 0, st>>>((const int64_t*)indptr, (const int32_t*)indices, plan, ntiles, c, r, b, bad);
+    spmv_pack_kernel<int32_t, int64_t, WRITE><<<grid, 256, 0, st>>>((const int64_t*)indptr, (const int32_t*)indices, plan, ntiles, c, r, b, stat, vals, vbytes, vb, dict);
   else if (pt == B2S_I32)
-    spmv_pack_kernel<int64_t, int32_t, WRITE><<<grid, 256, 0, st>>>((const int32_t*)indptr, (const int64_t*)indices, plan, ntiles, c, r, b, bad);
+    spmv_pack_kernel<int64_t, int32_t, WRITE><<<grid, 256, 0, st>>>((const int32_t*)indptr, (const int64_t*)indices, plan, ntiles, c, r, b, stat, vals, vbytes, vb, dict);
   else
-    spmv_pack_kernel<int64_t, int64_t, WRITE><<<grid, 256, 0, st>>>((const int64_t*)indptr, (const int64_t*)indices, plan, ntiles, c, r, b, bad);
+    spmv_pack_kernel<int64_t, int64_t, WRITE><<<grid, 256, 0, st>>>((const int64_t*)indptr, (const int64_t*)indices, plan, ntiles, c, r, b, stat, vals, vbytes, vb, dict);
   B2S_LAUNCH_CHECK();
   return B2S_OK;
 }
 
-// Sections of the packed-structure buffer: tile bases, columns, row offsets (each 16-byte aligned)
+// Distinct bit patterns of vals[0, n), per block: each block keeps up to kMaxDict + 1 of them in shared memory (the
+// one past kMaxDict only marks the overflow, after which the block stops) and writes them to tabs[block], their count
+// to counts[block].  A warp looks its values up in the table and, for the ones it misses, inserts them in turn under a
+// block lock held by lane 0.  The host merges the blocks' tables (dict_collect).
+constexpr int kDictBlocks = 1024;
+template <typename U>
+__global__ void __launch_bounds__(256)
+spmv_dict_kernel(const U* __restrict__ vals, int64_t n, unsigned long long* __restrict__ tabs, int* __restrict__ counts) {
+  constexpr int CAP = kMaxDict + 1;
+  __shared__ U tab[CAP];
+  __shared__ int cnt, lock;
+  if (threadIdx.x == 0) { cnt = 0; lock = 0; }
+  __syncthreads();
+  volatile U* vtab = tab;
+  volatile int* vcnt = &cnt;
+  const unsigned full = 0xffffffffu;
+  const int lane = threadIdx.x & 31;
+  const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+  for (int64_t base = warp * 128; base < n; base += nwarps * 128) {      // warp-uniform
+    if (__shfl_sync(full, *vcnt, 0) > kMaxDict) break;
+    U v[4];
+    bool in[4];
+#pragma unroll
+    for (int q = 0; q < 4; q++) {
+      const int64_t k = base + 32 * q + lane;
+      in[q] = k < n;
+      v[q] = in[q] ? vals[k] : (U)0;
+    }
+#pragma unroll
+    for (int q = 0; q < 4; q++) {
+      const int c = *vcnt;
+      bool hit = !in[q];
+      for (int i = 0; i < c && i < CAP && !hit; i++) hit = vtab[i] == v[q];
+      unsigned miss = __ballot_sync(full, !hit);
+      if (!miss) continue;
+      if (lane == 0) while (atomicCAS(&lock, 0, 1) != 0) {}
+      __syncwarp();
+      __threadfence_block();
+      while (miss) {
+        const U cand = __shfl_sync(full, v[q], __ffs(miss) - 1);
+        const int c2 = *vcnt;
+        bool found = false;
+        for (int i = 0; i < c2 && i < CAP; i++) found = found || vtab[i] == cand;
+        if (lane == 0 && !found && c2 < CAP) {
+          vtab[c2] = cand;
+          __threadfence_block();
+          *vcnt = c2 + 1;
+        }
+        __syncwarp();
+        miss &= ~__ballot_sync(full, in[q] && v[q] == cand);
+      }
+      __threadfence_block();
+      __syncwarp();
+      if (lane == 0) atomicExch(&lock, 0);
+    }
+  }
+  __syncthreads();
+  const int c = cnt < CAP ? cnt : CAP;
+  if ((int)threadIdx.x < c) tabs[(int64_t)blockIdx.x * CAP + threadIdx.x] = (unsigned long long)tab[threadIdx.x];
+  if (threadIdx.x == 0) counts[blockIdx.x] = cnt;
+}
+
+// Sections of the packed-structure buffer: tile bases, columns, row offsets, value dictionary (each 16-byte aligned)
 static inline int64_t round16(int64_t b) { return (b + 15) & ~(int64_t)15; }
+constexpr int64_t kDictBytes = kMaxDict * 8;
 static inline void pack_sizes(int64_t ntiles, int64_t nrows, int64_t nnz, int64_t* base_b, int64_t* cols_b,
                               int64_t* rows_b) {
   *base_b = round16(8 * ntiles);
@@ -225,8 +313,12 @@ struct PlanHandle {
   int64_t uniform_tiles, short_tiles;
   double lines_per_warp;
   int pack_ok;      // 1: every tile holds short rows inside a 65536-column window (b2s_spmv_plan_pack may pack it)
-  int use_packed;   // 1: launches stream `pk` (set by b2s_spmv_plan_pack; b2s_spmv_plan_set_packed toggles it)
-  PackedTiles pk;   // the packed structure in the caller's buffer (NULL until packed)
+  int64_t pack_w;   // widest column window (largest minus smallest column) of a tile, when pack_ok
+  int use_packed;   // 0: launches stream the CSR arrays; 1: `pk` and the values; 2: `pk` with coded values (when
+                    // launched with coded_vals); set by packing, b2s_spmv_plan_set_packed switches it
+  PackedTiles pk;   // the packed structure in the caller's buffer (NULL until packed; dict NULL unless coded)
+  const void* coded_vals;               // the values the codes were built from
+  unsigned char dict_img[kDictBytes];   // host copy of the dictionary written to the buffer
   const PlanEntry* dev;
   // row chunks for pipelined host<->device SpMV: chunk c = tiles [ctile[c], ctile[c+1]), rows [crow[c], crow[c+1]),
   // reading x only inside [ccol_lo[c], ccol_hi[c])
@@ -350,16 +442,21 @@ static int plan_create_impl(int vt, int it, int pt, int64_t nrows, int64_t ncols
   h->flavor = flavor;
   // 3. can the structure be packed?  Only for the streaming short-row configs, and only if every tile qualifies
   h->pack_ok = 0;
+  h->pack_w = 0;
   h->use_packed = 0;
-  h->pk = PackedTiles{nullptr, nullptr, nullptr};
+  h->pk = PackedTiles{nullptr, nullptr, nullptr, nullptr, 0, 0};
+  h->coded_vals = nullptr;
   if (flavor == 2 && cfg_packable(cfg, vt) && kCfgs[cfg].kind == 1 && ntiles > 0 && nnz > 0) {
-    B2S_CUDA(cudaMemsetAsync(stat, 0, 8, st));
-    if (int rc = launch_pack<false>(it, pt, indptr, indices, dev, ntiles, PackedTiles{nullptr, nullptr, nullptr}, stat, st))
+    B2S_CUDA(cudaMemsetAsync(stat, 0, 16, st));
+    if (int rc = launch_pack<false>(it, pt, indptr, indices, dev, ntiles, h->pk, stat, nullptr, 0, DictBits{}, st)) {
+      delete h;
       return rc;
-    unsigned long long bad = 1;
-    B2S_CUDA(cudaMemcpyAsync(&bad, stat, sizeof(bad), cudaMemcpyDeviceToHost, st));
+    }
+    unsigned long long bw[2] = {1, 0};
+    B2S_CUDA(cudaMemcpyAsync(bw, stat, sizeof(bw), cudaMemcpyDeviceToHost, st));
     B2S_CUDA(cudaStreamSynchronize(st));
-    h->pack_ok = bad == 0 ? 1 : 0;
+    h->pack_ok = bw[0] == 0 ? 1 : 0;
+    h->pack_w = (int64_t)bw[1];
   }
   h->nrows = nrows; h->ncols = ncols; h->nnz = nnz; h->ntiles = ntiles;
   h->uniform_tiles = uniform_tiles; h->short_tiles = short_tiles;
@@ -433,41 +530,125 @@ int b2s_spmv_plan_destroy(void* plan) {
   return B2S_OK;
 }
 
-/* Size of the device buffer b2s_spmv_plan_pack needs; 0 when the matrix does not qualify for the packed kernel */
+/* Size of the device buffer b2s_spmv_plan_pack / _pack_coded need; 0 when the matrix does not qualify for the packed
+ * kernel */
 int64_t b2s_spmv_plan_pack_bytes(const void* plan) {
   const PlanHandle* h = (const PlanHandle*)plan;
   if (!h || h->magic != kPlanMagic || !h->pack_ok) return 0;
   int64_t b, c, r;
   pack_sizes(h->ntiles, h->nrows, h->nnz, &b, &c, &r);
-  return b + c + r;
+  return b + c + r + kDictBytes;
+}
+
+// The sorted distinct bit patterns of vals[0, nnz) into *d; false when there are more than kMaxDict.  One pass over
+// the values; the per-block tables come back to the host (at most kDictBlocks x 17 patterns) and are merged there.
+static int dict_collect(int vt, int64_t nnz, const void* vals, cudaStream_t st, DictBits* d, bool* fits) {
+  constexpr int CAP = kMaxDict + 1;
+  *fits = false;
+  d->n = 0;
+  const int64_t blocks64 = (nnz + 1023) / 1024;
+  const int blocks = (int)(blocks64 < kDictBlocks ? blocks64 : kDictBlocks);
+  if (blocks <= 0) return B2S_OK;
+  unsigned char* tmp = nullptr;
+  const size_t tab_b = sizeof(unsigned long long) * CAP * (size_t)blocks;
+  B2S_CUDA(cudaMallocAsync((void**)&tmp, tab_b + sizeof(int) * (size_t)blocks, st));
+  unsigned long long* tabs = (unsigned long long*)tmp;
+  int* counts = (int*)(tmp + tab_b);
+  if (vt == B2S_F64) spmv_dict_kernel<unsigned long long><<<blocks, 256, 0, st>>>((const unsigned long long*)vals, nnz, tabs, counts);
+  else               spmv_dict_kernel<unsigned><<<blocks, 256, 0, st>>>((const unsigned*)vals, nnz, tabs, counts);
+  cudaError_t le = cudaGetLastError();
+  std::vector<unsigned long long> host_tabs((size_t)CAP * blocks);
+  std::vector<int> host_counts(blocks);
+  if (le == cudaSuccess) le = cudaMemcpyAsync(host_tabs.data(), tabs, tab_b, cudaMemcpyDeviceToHost, st);
+  if (le == cudaSuccess) le = cudaMemcpyAsync(host_counts.data(), counts, sizeof(int) * blocks, cudaMemcpyDeviceToHost, st);
+  if (le == cudaSuccess) le = cudaStreamSynchronize(st);
+  cudaFreeAsync(tmp, st);
+  B2S_CUDA(le);
+  std::vector<unsigned long long> all;
+  for (int b = 0; b < blocks; b++) {
+    if (host_counts[b] > kMaxDict) return B2S_OK;
+    all.insert(all.end(), host_tabs.begin() + (size_t)CAP * b, host_tabs.begin() + (size_t)CAP * b + host_counts[b]);
+  }
+  std::sort(all.begin(), all.end());
+  all.erase(std::unique(all.begin(), all.end()), all.end());
+  if (all.size() > (size_t)kMaxDict) return B2S_OK;
+  for (size_t i = 0; i < all.size(); i++) d->v[i] = all[i];
+  d->n = (int)all.size();
+  *fits = true;
+  return B2S_OK;
+}
+
+// Fills the packed buffer (coded when vals != NULL, see PackedTiles) and switches the plan's launches to it.
+static int pack_write(PlanHandle* h, const void* indptr, const void* indices, const void* vals, int vb,
+                      const DictBits& dict, void* buf_dev, cudaStream_t st) {
+  int64_t b, c, r;
+  pack_sizes(h->ntiles, h->nrows, h->nnz, &b, &c, &r);
+  unsigned char* p = (unsigned char*)buf_dev;
+  const bool coded = vals != nullptr;
+  const int sv = h->vt == B2S_F32 ? 4 : 8;
+  PackedTiles pk{(const uint16_t*)(p + b), (const uint16_t*)(p + b + c), (const long long*)p,
+                 coded ? (const void*)(p + b + c + r) : nullptr, coded ? vb : 0, coded ? dict.n : 0};
+  B2S_CUDA(cudaMemsetAsync(buf_dev, 0, (size_t)(b + c + r + kDictBytes), st));
+  if (coded) {
+    memset(h->dict_img, 0, sizeof(h->dict_img));
+    for (int i = 0; i < dict.n; i++) {
+      if (sv == 8) memcpy(h->dict_img + 8 * i, &dict.v[i], 8);
+      else { const uint32_t v32 = (uint32_t)dict.v[i]; memcpy(h->dict_img + 4 * i, &v32, 4); }
+    }
+    B2S_CUDA(cudaMemcpyAsync(p + b + c + r, h->dict_img, sizeof(h->dict_img), cudaMemcpyHostToDevice, st));
+  }
+  if (int rc = launch_pack<true>(h->it, h->pt, indptr, indices, h->dev, h->ntiles, pk, nullptr, vals, coded ? sv : 0,
+                                 dict, st))
+    return rc;
+  h->pk = pk;
+  h->coded_vals = vals;
+  h->use_packed = coded ? 2 : 1;
+  return B2S_OK;
+}
+
+static int pack_check(const PlanHandle* h, const void* indptr, const void* indices, const void* buf_dev) {
+  B2S_CHECK_ARG(h && h->magic == kPlanMagic, "bad plan handle");
+  B2S_CHECK_ARG(h->pack_ok, "this plan does not qualify for packing (b2s_spmv_plan_pack_bytes returns 0)");
+  B2S_CHECK_ARG(indptr && indices, "indptr / indices is NULL");
+  B2S_CHECK_ARG(buf_dev != nullptr && aligned16(buf_dev), "pack buffer must be non-NULL and 16-byte aligned");
+  return B2S_OK;
 }
 
 /* Packs the structure of a qualifying plan into buf_dev (b2s_spmv_plan_pack_bytes bytes, 16-byte aligned, caller-owned
  * and kept alive as long as the plan is used); later launches with the plan stream the packed form. */
 int b2s_spmv_plan_pack(void* plan, const void* indptr, const void* indices, void* buf_dev, void* stream) {
   PlanHandle* h = (PlanHandle*)plan;
-  B2S_CHECK_ARG(h && h->magic == kPlanMagic, "bad plan handle");
-  B2S_CHECK_ARG(h->pack_ok, "this plan does not qualify for packing (b2s_spmv_plan_pack_bytes returns 0)");
-  B2S_CHECK_ARG(indptr && indices, "indptr / indices is NULL");
-  B2S_CHECK_ARG(buf_dev != nullptr && aligned16(buf_dev), "pack buffer must be non-NULL and 16-byte aligned");
-  cudaStream_t st = (cudaStream_t)stream;
-  int64_t b, c, r;
-  pack_sizes(h->ntiles, h->nrows, h->nnz, &b, &c, &r);
-  unsigned char* p = (unsigned char*)buf_dev;
-  PackedTiles pk{(const uint16_t*)(p + b), (const uint16_t*)(p + b + c), (const long long*)p};
-  B2S_CUDA(cudaMemsetAsync(buf_dev, 0, (size_t)(b + c + r), st));
-  if (int rc = launch_pack<true>(h->it, h->pt, indptr, indices, h->dev, h->ntiles, pk, nullptr, st)) return rc;
-  h->pk = pk;
-  h->use_packed = 1;
-  return B2S_OK;
+  if (int rc = pack_check(h, indptr, indices, buf_dev)) return rc;
+  return pack_write(h, indptr, indices, nullptr, 0, DictBits{}, buf_dev, (cudaStream_t)stream);
 }
 
-/* tools / tests: 1 = launches stream the packed structure (the plan must have been packed), 0 = the CSR arrays */
-int b2s_spmv_plan_set_packed(void* plan, int on) {
+/* b2s_spmv_plan_pack, and when `vals` holds at most 16 distinct bit patterns and every tile's column window leaves
+ * room for their codes, also codes the values into the column words: launches with this `vals` pointer then stream no
+ * values.  The plan is then only valid while indptr, indices AND vals are unchanged. */
+int b2s_spmv_plan_pack_coded(void* plan, const void* indptr, const void* indices, const void* vals, void* buf_dev,
+                             void* stream) {
+  PlanHandle* h = (PlanHandle*)plan;
+  if (int rc = pack_check(h, indptr, indices, buf_dev)) return rc;
+  B2S_CHECK_ARG(vals != nullptr, "vals is NULL");
+  cudaStream_t st = (cudaStream_t)stream;
+  DictBits d{};
+  bool fits = false;
+  if (int rc = dict_collect(h->vt, h->nnz, vals, st, &d, &fits)) return rc;
+  int vb = 0;
+  while ((1 << vb) < d.n) vb++;
+  const bool coded = fits && h->pack_w < (1LL << (16 - vb));
+  return pack_write(h, indptr, indices, coded ? vals : nullptr, vb, d, buf_dev, st);
+}
+
+/* tools / tests: 0 = launches stream the CSR arrays, 1 = the packed structure and the values, 2 = the packed structure
+ * with coded values (the plan must have been packed / coded) */
+int b2s_spmv_plan_set_packed(void* plan, int mode) {
   PlanHandle* h = (PlanHandle*)plan;
   B2S_CHECK_ARG(h && h->magic == kPlanMagic, "bad plan handle");
-  B2S_CHECK_ARG(!on || h->pk.cols != nullptr, "the plan has not been packed (b2s_spmv_plan_pack)");
-  h->use_packed = on ? 1 : 0;
+  B2S_CHECK_ARG(mode >= 0 && mode <= 2, "mode must be 0, 1 or 2");
+  B2S_CHECK_ARG(!mode || h->pk.cols != nullptr, "the plan has not been packed (b2s_spmv_plan_pack)");
+  B2S_CHECK_ARG(mode != 2 || h->pk.dict != nullptr, "the plan's values are not coded (b2s_spmv_plan_pack_coded)");
+  h->use_packed = mode;
   return B2S_OK;
 }
 
@@ -476,14 +657,14 @@ static bool plan_runs_packed(const PlanHandle* h) {
 }
 
 /* out[0] = tile config, out[1] = bit0 row-group kernel forced, bit1 uniform-row flavour, bit2 scattered, bit3 short-row
- * flavour, bit4 TMA kind, bit5 packed structure; out[2] = ntiles, out[3] = 1000 * mean distinct x lines per 32
- * consecutive nonzeros */
+ * flavour, bit4 TMA kind, bit5 packed structure, bit6 coded values, bits 8..12 distinct values of a coded plan;
+ * out[2] = ntiles, out[3] = 1000 * mean distinct x lines per 32 consecutive nonzeros */
 int b2s_spmv_plan_info(const void* plan, int64_t* out4_host) {
   const PlanHandle* h = (const PlanHandle*)plan;
   B2S_CHECK_ARG(h && h->magic == kPlanMagic && out4_host, "bad plan handle / out pointer");
   out4_host[0] = h->cfg;
   out4_host[1] = h->use_rowgroup + 2 * (h->flavor == 1) + 4 * h->scattered + 8 * (h->flavor == 2) + 16 * (kCfgs[h->cfg].kind == 1) +
-                 32 * plan_runs_packed(h);
+                 32 * plan_runs_packed(h) + 64 * (plan_runs_packed(h) && h->use_packed == 2) + 256 * (int64_t)h->pk.ndict;
   out4_host[2] = h->ntiles;
   out4_host[3] = (int64_t)(h->lines_per_warp * 1000.0);
   return B2S_OK;
@@ -554,7 +735,10 @@ static int spmv_impl(int vt, int it, int pt, int64_t nrows, int64_t ncols, int64
   B2S_CHECK_ARG((a.tile_lo == 0 && a.tile_hi == h->ntiles) || tma, "tile sub-ranges need a TMA tile plan");
   if (a.tile_lo == a.tile_hi && !order) return B2S_OK;
   a.nrows = nrows; a.nnz = nnz;
-  a.pk = plan_runs_packed(h) ? h->pk : PackedTiles{nullptr, nullptr, nullptr};
+  a.pk = plan_runs_packed(h) ? h->pk : PackedTiles{nullptr, nullptr, nullptr, nullptr, 0, 0};
+  // the coded kernel only for the values the codes were built from; any other `vals` is streamed (still decoding the
+  // column words with vb)
+  if (h->use_packed != 2 || vals != h->coded_vals) a.pk.dict = nullptr;
   a.indptr = indptr; a.indices = indices; a.vals = vals; a.x = x; a.y = y;
   a.plan = h->dev;
   a.vec_ok = aligned ? 1 : 0;

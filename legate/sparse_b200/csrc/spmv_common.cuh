@@ -70,6 +70,11 @@ static constexpr int kScatterShortCfgF64 = 13;
 static constexpr bool cfg_packable(int c, int vt) {
   return vt == B2S_F32 ? c == kDefaultCfgF32 : c == kShortCfgF64;
 }
+// Stage ring depth and CTAs/SM of the coded packed kernel.  Without values a stage holds 4.1 KB (fp64) instead of
+// 12.3 KB, so it takes more stages to keep as many bytes in flight: on the H100 (700 W) 4 stages beat 2, 3 and 6 for
+// both value types (DESIGN.md 8).  The CTAs/SM stay those of the uncoded shapes: the fp64 kernel needs 63-64 registers.
+static constexpr int kCodedStagesF64 = 4, kCodedMinbF64 = 6;
+static constexpr int kCodedStagesF32 = 4, kCodedMinbF32 = 8;
 
 static inline int cfg_cap(int c, int vt) {
   const TileCfgRt& k = kCfgs[c];
@@ -112,10 +117,17 @@ struct TileOrder {
 //   rows[r0 + 8 t + j] = indptr[r0 + j] - kb   for j in [0, nr]               (uint16; kb = k0 rounded down to 4)
 // The gaps of 16 / 8 entries between consecutive tiles let each tile's slice start and end on a 16-byte boundary, so
 // the producer bulk-copies [k0 & ~7, round8(kce)) + 16 t and [(r0 + 8 t) & ~7, round8(r1 + 8 t + 1)) of them.
+// Coded values (b2s_spmv_plan_pack_coded): when `vals` holds at most kMaxDict distinct bit patterns and every tile's
+// window fits in 16 - vb bits, each column word is (indices[k] - base[t]) << vb | code, vals[k] = dict[code], and the
+// coded kernel streams no values at all; a launch of the packed kernel with streamed values decodes the columns as
+// w >> vb too.  Uncoded plans have vb = 0 and dict = NULL.
+constexpr int kMaxDict = 16;
 struct PackedTiles {
   const uint16_t* cols;
   const uint16_t* rows;
   const long long* base;   // smallest column of each tile
+  const void* dict;        // kMaxDict values (sorted bit patterns, the first ndict used); NULL = values are streamed
+  int vb, ndict;           // code bits per column word, distinct values
 };
 constexpr int kPackColGap = 16, kPackRowGap = 8;
 

@@ -540,7 +540,7 @@ class dist_csr_array:
                     flags = []
                 desc = _ops.fuse_desc(ranges, n_free, flags=flags, sends=sends, acks=acks, epoch_ctr=pc.epoch_ctr,
                                       ticket=pc.ticket, epoch_add=1, epoch_bump=1, error=pc.error_word)
-                info = {"mode": "halo", "desc": desc, "plan": plan, "pc": pc}
+                info = {"mode": "halo", "desc": desc, "pc": pc}
         elif self.exchange_mode == "allgather":
             ok = bool(usable and self.col_plan.uniform)
             # Column blocks pay per-block launch / row-pointer / y read-modify-write overheads (tools/bench_blocks.py
@@ -555,7 +555,7 @@ class dist_csr_array:
                 if ok:
                     sends = [(q, lo, pc.peer_x_off[q] + lo, hi - lo) for q in range(self.nranks) if q != self.rank and hi > lo]
                     slice_bytes = (hi - lo) * item
-                    info = {"mode": "gather", "sends": sends, "pc": pc, "plan": A._get_plan(),
+                    info = {"mode": "gather", "sends": sends, "pc": pc,
                             "recv_peers": [q for q in range(self.nranks) if q != self.rank],
                             "cps": 16 if slice_bytes >= (1 << 22) else (4 if slice_bytes >= (1 << 18) else 1)}
             elif self._agree(ok):
@@ -573,7 +573,8 @@ class dist_csr_array:
                                               ticket=pc.ticket, epoch_add=0, epoch_bump=0, error=pc.error_word,
                                               accumulate=True)
                 slice_bytes = (hi - lo) * item
-                info = {"mode": "blocks", "blocks": blocks, "descs": descs, "sends": sends, "recv_peers": recv_peers,
+                info = {"mode": "blocks", "blocks": blocks, "blocks_of": (A._data.data_ptr(), A._data._version),
+                        "descs": descs, "sends": sends, "recv_peers": recv_peers,
                         "pc": pc, "cps": 16 if slice_bytes >= (1 << 22) else (4 if slice_bytes >= (1 << 18) else 1),
                         "order": [(self.rank + d) % self.nranks for d in range(1, self.nranks)]}
         self._fused[key] = info
@@ -601,9 +602,11 @@ class dist_csr_array:
         return out
 
     def _dot_fused(self, info, A, x_full, out, w=None, dot_out=None):
+        # the plan is looked up per launch, not kept in `info`: a coded plan holds the values, so an in-place edit of
+        # A.data must reach the launch through a new plan (same structure: the same tiles the descriptors name)
         xin = x_full[: A.shape[1]]
         if info["mode"] == "halo":
-            _ops.spmv_fused(A.indptr, A.indices, A.data, xin, out, A.shape, info["plan"], info["desc"], w=w, dot_out=dot_out)
+            _ops.spmv_fused(A.indptr, A.indices, A.data, xin, out, A.shape, A._get_plan(), info["desc"], w=w, dot_out=dot_out)
             return out
         pc = info["pc"]
         if info["mode"] == "gather":
@@ -611,10 +614,14 @@ class dist_csr_array:
             _ops.peer_push(x_full, self.rank, pc.peers, info["sends"], info["recv_peers"], info["cps"])
             _ops.peer_push_wait(self.rank, pc.peers, info["recv_peers"])
             if w is not None:
-                _ops.spmv_dot(A.indptr, A.indices, A.data, xin, out, w, dot_out, A.shape, info["plan"])
+                _ops.spmv_dot(A.indptr, A.indices, A.data, xin, out, w, dot_out, A.shape, A._get_plan())
             else:
-                _ops.spmv(A.indptr, A.indices, A.data, xin, out, A.shape, plan=info["plan"])
+                _ops.spmv(A.indptr, A.indices, A.data, xin, out, A.shape, plan=A._get_plan())
             return out
+        if info["blocks_of"] != (A._data.data_ptr(), A._data._version):
+            # the column blocks hold copies of the values: cut them again (same structure, so the same tiles)
+            info["blocks"] = self._column_blocks(A)
+            info["blocks_of"] = (A._data.data_ptr(), A._data._version)
         cur = torch.cuda.current_stream()
         if getattr(self, "_comm_stream", None) is None:
             self._comm_stream = torch.cuda.Stream()
@@ -699,12 +706,16 @@ class dist_csr_array:
 
         key = (x_full.data_ptr(), out.data_ptr(), os.environ.get("B2S_OVERLAP", "0"))
         cache = self.__dict__.setdefault("_dot_graphs", {})
-        g = cache.get(key)
+        # a graph replays the launches of the plan it was captured with (which may hold coded values of local.data):
+        # it is only valid while that plan is the current one, and keeps it -- and its pack buffer -- alive
+        plan = self.local._get_plan()
+        hit = cache.get(key)
+        g = hit[0] if hit is not None and hit[1] is plan else None
         if g is None:
             self.dot(x_full, out=out)  # eager warm-up: plans, schedules, communicators, kernel attributes
             torch.cuda.synchronize()
             g = _try_capture(lambda: self.dot(x_full, out=out)) or False
-            cache[key] = g
+            cache[key] = (g, plan)
         if g:
             g.replay()
         else:

@@ -1,12 +1,13 @@
-"""Kernel-level A/B of the packed SpMV structure against the CSR-streaming kernel, next to a streaming ceiling.
+"""Kernel-level A/B/C of the SpMV structure encodings -- coded values, packed structure, CSR arrays -- next to a streaming
+ceiling.
 
     python tools/bench_packed.py [--launches 200] [--reps 5] [--out DIR]
 
 One process, one GPU.  The cases run in alternation, round after round (so drift on a shared machine hits all of them
 alike), each timed with CUDA events around `--launches` back-to-back launches:
-  * the 5-point Laplacian on a 3162 x 3162 grid (the benchmark's operator) in fp64, packed and unpacked (the plan hook
-    b2s_spmv_plan_set_packed switches the same plan), and in fp32;
-  * an 11-per-row band of 10M rows, fp64, packed and unpacked;
+  * the 5-point Laplacian on a 3162 x 3162 grid (the benchmark's operator) in fp64, with coded values, packed with
+    streamed values, and unpacked (the plan hook b2s_spmv_plan_set_packed switches the same plan), and in fp32;
+  * an 11-per-row band of 10M rows, fp64, the same three ways;
   * a read-only streaming probe: torch.sum over 1.6 GB of fp64 -- the bandwidth this card sustains at its power limit.
 Per case: median / min / max time per launch, the CSR-equivalent rate (the bytes CSR SpMV needs, what bench.py
 counts), the bytes the launched kernel actually moves (from the plan's tile shapes) and that rate as a fraction of the
@@ -43,9 +44,9 @@ def csr_bytes(A):
     return A.nnz * (sv + si) + (n + 1) * sp + m * sv + n * sv
 
 
-def moved_bytes(A, plan, packed):
+def moved_bytes(A, plan, mode):
     """Bytes one launch streams: per tile the plan entry, and either the staged 16-byte groups of indices / indptr or
-    the packed uint16 slices plus the tile base; values, x once and y once."""
+    the packed uint16 slices plus the tile base; values (none when coded: mode 2), x once and y once."""
     sv, si, sp = A.data.element_size(), A.indices.element_size(), A.indptr.element_size()
     n, m = A.shape
     e = plan.buf[: 4 * (plan.tiles + 1)].view(-1, 4).cpu().numpy().astype(np.int64)
@@ -54,13 +55,13 @@ def moved_bytes(A, plan, packed):
     t = np.arange(plan.tiles)
     k0, k1, r0, r1 = k[:-1], k[1:], r[:-1], r[1:]
     live = r1 > r0
-    if packed:
+    if mode:
         c = ((k1 + 7) & ~7) - (k0 & ~7)
         q = ((r1 + 1 + 8 * t + 7) & ~7) - ((r0 + 8 * t) & ~7)
         struct = int(((c + q) * 2 + 8)[live].sum())
     else:
         struct = int(((k1 - (k0 & ~3)) * si)[live].sum() + ((((r1 + 1 + 3) & ~3) - (r0 & ~3)) * sp)[live].sum())
-    return A.nnz * sv + struct + 16 * plan.tiles + m * sv + n * sv
+    return (0 if mode == 2 else A.nnz * sv) + struct + 16 * plan.tiles + m * sv + n * sv
 
 
 def time_per_launch(fn, launches):
@@ -97,12 +98,12 @@ def main():
         def run(A=A, plan=plan, x=x, y=y):
             _ops.spmv(A.indptr, A.indices, A.data, x, y, A.shape, plan=plan)
 
-        for packed in ([True, False] if plan.packed else [False]):
-            cases[f"{name}_{'packed' if packed else 'csr'}"] = dict(
-                run=run, plan=plan, packed=packed, csr=csr_bytes(A), moved=moved_bytes(A, plan, packed),
+        for mode in ([2, 1, 0] if plan.coded else [1, 0] if plan.packed else [0]):
+            cases[f"{name}_{('csr', 'packed', 'coded')[mode]}"] = dict(
+                run=run, plan=plan, mode=mode, csr=csr_bytes(A), moved=moved_bytes(A, plan, mode),
                 flops=2 * A.nnz, kernel=None)
     probe = torch.rand(200_000_000, dtype=torch.float64, device="cuda")   # 1.6 GB
-    cases["probe_sum_fp64_1.6GB"] = dict(run=lambda: probe.sum(), plan=None, packed=False, csr=None,
+    cases["probe_sum_fp64_1.6GB"] = dict(run=lambda: probe.sum(), plan=None, mode=0, csr=None,
                                          moved=probe.numel() * 8, flops=None, kernel="torch.sum")
 
     def select(c):
@@ -110,7 +111,7 @@ def main():
         if plan is None:
             return
         if plan.pack_buf is not None:
-            plan.set_packed(c["packed"])
+            plan.set_packed(c["mode"])
         c["kernel"] = plan.kernel_name
 
     for c in cases.values():       # warm-up: module load, first-touch of every buffer
@@ -144,6 +145,9 @@ def main():
     for m in mats:
         if f"{m}_packed" in rows:
             print(f"# {m}: csr / packed time = {rows[f'{m}_csr']['us_median'] / rows[f'{m}_packed']['us_median']:.3f}")
+        if f"{m}_coded" in rows:
+            print(f"# {m}: packed / coded time = {rows[f'{m}_packed']['us_median'] / rows[f'{m}_coded']['us_median']:.3f}, "
+                  f"csr / coded = {rows[f'{m}_csr']['us_median'] / rows[f'{m}_coded']['us_median']:.3f}")
     if args.out:
         os.makedirs(args.out, exist_ok=True)
         with open(os.path.join(args.out, "bench_packed.json"), "w") as f:
