@@ -33,6 +33,8 @@
 //            streams those instead of indices / indptr -- 14.7 % fewer bytes for the 5-point Laplacian in fp64.
 //   coded   : when the values also take at most 16 distinct bit patterns, the spare high bits of the column words
 //            carry a value code and no values are streamed (59 % fewer bytes again for the Laplacian in fp64).
+//   row pairs: a packed tile of rows with at most 5 entries and 129..256 rows gives each lane two rows whose gathers are
+//            all issued before the first FMA -- one dependent trip per tile instead of two rounds.
 //
 // HBM-bound by construction: algorithmic bytes per launch are
 //   nnz*(sizeof V + sizeof I) + (nrows+1)*sizeof P + ncols*sizeof V + nrows*sizeof V.
@@ -394,6 +396,47 @@ __device__ __forceinline__ V short_row_sum(const C* __restrict__ scols, const V*
   return acc;
 }
 
+// short_row_sum for two rows of at most U entries each, in one round: the gathers of both rows are issued before the first
+// FMA, so a lane that owns two rows of a tile waits for one dependent trip to L2 instead of two.  Each row's sum is
+// formed exactly as short_row_sum forms it (U terms, left to right, zero for the slots past the row's end).
+template <int U, int XL, bool CODED, typename V, typename I, typename C>
+__device__ __forceinline__ void short_row_pair(const C* __restrict__ scols, const V* __restrict__ svals,
+                                               const V* __restrict__ x, int s0, int e0, int s1, int e1, I cbase,
+                                               int vb, V& sum0, V& sum1) {
+  I c[2][U];
+  V a[2][U];
+#pragma unroll
+  for (int r = 0; r < 2; r++) {
+#pragma unroll
+    for (int q = 0; q < U; q++) {
+      const int p = (r ? s1 : s0) + q;
+      const bool in = p < (r ? e1 : e0);
+      if constexpr (sizeof(C) == 2) {
+        const unsigned wd = in ? (unsigned)scols[p] : 0u;
+        c[r][q] = in ? cbase + (I)(wd >> vb) : (I)0;
+        if constexpr (CODED) a[r][q] = in ? svals[wd & ((1u << vb) - 1u)] : (V)0;
+        else                 a[r][q] = in ? svals[p] : (V)0;
+      } else {
+        c[r][q] = in ? scols[p] : (I)0;
+        a[r][q] = in ? svals[p] : (V)0;
+      }
+    }
+  }
+  V xv[2][U];
+#pragma unroll
+  for (int r = 0; r < 2; r++) {
+#pragma unroll
+    for (int q = 0; q < U; q++) xv[r][q] = ((r ? s1 : s0) + q < (r ? e1 : e0)) ? ld_x<XL>(x + c[r][q]) : (V)0;
+  }
+  V acc0 = (V)0, acc1 = (V)0;
+#pragma unroll
+  for (int q = 0; q < U; q++) acc0 += a[0][q] * xv[0][q];
+#pragma unroll
+  for (int q = 0; q < U; q++) acc1 += a[1][q] * xv[1][q];
+  sum0 = acc0;
+  sum1 = acc1;
+}
+
 // FLAVOR 0: generic reduce only (irregular long rows); 1: + uniform-row register path and bank-skewed reduce;
 // 2: + one-lane-per-row path for tiles of short rows.  PACKED (flavour 2 only, every tile short): the producer streams
 // the uint16 columns and row offsets of `pk` in place of indices / indptr; values and arithmetic are unchanged.
@@ -624,6 +667,32 @@ spmv_tma_kernel(TileOrder order, int64_t nrows, int64_t nnz, const P* __restrict
         const V* avals = CODED ? sdict : svals;   // where short_row_sum reads the values
         // packed row offsets are already relative to kb; the tile's first one is entry (r0 + 8 t) & 7 = r0 & 7
         const uint16_t* prow = reinterpret_cast<const uint16_t*>(st + LY::COLS_B + LY::VALS_B) + (r0 & 7);
+        // packed tiles of rows with at most 5 entries and more rows than consumer lanes (the 5-point Laplacian: ~170
+        // rows per fp64 tile, ~255 per fp32 tile, over 128 lanes): each lane takes rows j and j + CT together, one trip
+        // for both instead of one per round.  Same sums, same order of y stores and of the dot terms.
+        if (PACKED && !remote_tile && maxlen <= 5 && nr > CT && nr <= 2 * CT) {
+          const int j = ctid, j2 = ctid + CT;
+          const bool live2 = j2 < nr;
+          const int sa = prow[j], ea = prow[j + 1];
+          const int sb = live2 ? (int)prow[j2] : 0, eb = live2 ? (int)prow[j2 + 1] : 0;
+          const V yold = acc_y ? __ldcg(y + r0 + j) : (V)0;
+          const V yold2 = (acc_y && live2) ? __ldcg(y + r0 + j2) : (V)0;
+          V sum, sum2;
+          if (maxlen <= 4) short_row_pair<4, XL, CODED>(tcols, avals, x, sa, ea, sb, eb, cbase, vb, sum, sum2);
+          else             short_row_pair<5, XL, CODED>(tcols, avals, x, sa, ea, sb, eb, cbase, vb, sum, sum2);
+          sum += yold;
+          y[r0 + j] = sum;
+          if (DOT) dot_acc += (double)sum * (double)w[r0 + j];
+          if (live2) {
+            sum2 += yold2;
+            y[r0 + j2] = sum2;
+            if (DOT) dot_acc += (double)sum2 * (double)w[r0 + j2];
+          }
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&empty[s]);
+          it++;
+          continue;
+        }
         for (int j0 = ctid - lane; j0 < nr; j0 += CT) {      // warp-uniform trip count (the round count below is per warp)
           const int j = j0 + lane;
           const bool live = j < nr;
