@@ -320,6 +320,42 @@ int         b2s_coo_to_csr(int vt, int it, int pt, int64_t nrows, int64_t nnz, c
 int         b2s_csr_transpose(int vt, int it, int pt, int64_t nrows, int64_t ncols, int64_t nnz,
                               const void* indptr, const void* indices, const void* vals,
                               void* t_indptr, void* t_indices, void* t_vals, void* scratch, void* stream);
+/* Sort every row of a CSR matrix by column in place (the row sort of the two calls above; repeated columns stay
+ * adjacent in unspecified order).  `scratch`: b2s_convert_scratch_bytes(nrows, pt) bytes.  Syncs the stream once. */
+int         b2s_csr_sort_rows(int vt, int it, int pt, int64_t nrows, int64_t nnz, const void* indptr, void* indices,
+                              void* vals, void* scratch, void* stream);
+
+/* ---- elementwise: C = A op B for two CSR matrices of the same shape (m x n) ----------------------------------
+ * Replaces the reference's add() (sparse/csr.py:760-776, 972-1030: a per-row nnz task + cuSPARSE csrgeam2,
+ * src/sparse/array/csr/add.cu) and mult() (csr.py:1033-1099, mult.cu).  A and B share vt / it / pt; rows must be
+ * non-decreasing in column (repeated columns are summed in stored order before the op).  The structure is symbolic:
+ * C's row is the union (ADD, SUB) or intersection (MUL) of the two rows' column sets, no entry is dropped for being
+ * zero.  Values: ADD a+b / a / b, SUB a-b / a / -b, MUL a*b.
+ * Pass 1 (symbolic): c_indptr[m+1] (int64); info_host[0] = nnz(C), info_host[1] / [2] = 1 when some row of A / B has
+ *   decreasing columns (the structure is then meaningless: sort the rows, b2s_csr_sort_rows, and start again).  Syncs.
+ * Pass 2 (numeric): c_indices (width it, strictly increasing within a row) and c_vals.
+ * `scratch`: b2s_csr_binop_scratch_bytes(m) bytes, passed unchanged from pass 1 to pass 2. */
+#define B2S_EW_ADD 0
+#define B2S_EW_SUB 1
+#define B2S_EW_MUL 2
+int64_t     b2s_csr_binop_scratch_bytes(int64_t m);
+int         b2s_csr_binop_symbolic(int op, int it, int pt, int64_t m, int64_t n,
+                                   const void* a_indptr, const void* a_indices,
+                                   const void* b_indptr, const void* b_indices,
+                                   int64_t* c_indptr, int64_t* info_host /*[3]*/, void* scratch, void* stream);
+int         b2s_csr_binop_numeric(int op, int vt, int it, int pt, int64_t m, int64_t n,
+                                  const void* a_indptr, const void* a_indices, const void* a_vals,
+                                  const void* b_indptr, const void* b_indices, const void* b_vals,
+                                  const int64_t* c_indptr, void* c_indices, void* c_vals, void* scratch, void* stream);
+/* out_vals[p] = vals[p] * D with A's structure (reference mult_dense, csr.py:1102-1148, and the row / column
+ * broadcasts of multiply): ROWS D[row] (m entries), COLS D[col] (n entries), DENSE D[row * ldd + col] (row-major m x n,
+ * ldd >= n).  out_vals may alias vals. */
+#define B2S_SCALE_ROWS  0
+#define B2S_SCALE_COLS  1
+#define B2S_SCALE_DENSE 2
+int         b2s_csr_scale(int vt, int it, int pt, int64_t m, int64_t n, int64_t nnz, int mode,
+                          const void* indptr, const void* indices, const void* vals,
+                          const void* d, int64_t ldd, void* out_vals, void* stream);
 
 /* ---- multi-GPU: NCCL communicator owned by the library (SURVEY 8b) -----------------------------------------
  * For hosts without torch.distributed (and for multi-node runs): the library binds NCCL at run time (dlopen of

@@ -78,6 +78,14 @@ SIGNATURES = {
     "b2s_convert_scratch_bytes": (c_i64, [c_i64, c_i32]),
     "b2s_coo_to_csr": (c_i32, [c_i32, c_i32, c_i32, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "b2s_csr_transpose": (c_i32, [c_i32, c_i32, c_i32, c_i64, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "b2s_csr_sort_rows": (c_i32, [c_i32, c_i32, c_i32, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "b2s_csr_binop_scratch_bytes": (c_i64, [c_i64]),
+    "b2s_csr_binop_symbolic": (c_i32, [c_i32, c_i32, c_i32, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
+                                       c_vp]),
+    "b2s_csr_binop_numeric": (c_i32, [c_i32, c_i32, c_i32, c_i32, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
+                                      c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "b2s_csr_scale": (c_i32, [c_i32, c_i32, c_i32, c_i64, c_i64, c_i64, c_i32, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp,
+                              c_vp]),
     "b2s_comm_nccl_version": (c_i32, []),
     "b2s_comm_unique_id": (c_i32, [c_vp]),
     "b2s_comm_init": (c_i32, [c_i32, c_i32, c_vp, ctypes.POINTER(c_vp)]),

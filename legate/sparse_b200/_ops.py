@@ -329,6 +329,65 @@ def csr_transpose(indptr, indices, data, shape):
     return t_indptr, t_indices, t_vals
 
 
+def csr_sort_rows(indptr, indices, data):
+    """Sort every row of (indptr, indices, data) by column IN PLACE through b2s_csr_sort_rows; returns (indices, data)."""
+    _chk_dev(indptr, indices, data)
+    assert indices.is_contiguous() and data.is_contiguous()
+    nrows = indptr.shape[0] - 1
+    pt = idx_code(indptr.dtype)
+    scratch = torch.empty(int(L.b2s_convert_scratch_bytes(nrows, pt)), dtype=torch.uint8, device=data.device)
+    _lib.check(L.b2s_csr_sort_rows(vt_code(data.dtype), idx_code(indices.dtype), pt, nrows, int(data.shape[0]),
+                                   ptr(indptr), ptr(indices), ptr(data), ptr(scratch), _stream()), "b2s_csr_sort_rows")
+    return indices, data
+
+
+# ---- elementwise ------------------------------------------------------------------------------------------------
+EW_OPS = {"add": 0, "sub": 1, "mul": 2}       # B2S_EW_ADD / _SUB / _MUL
+SCALE_MODES = {"rows": 0, "cols": 1, "dense": 2}   # B2S_SCALE_ROWS / _COLS / _DENSE
+
+
+def csr_binop(op: str, a_indptr, a_indices, a_data, b_indptr, b_indices, b_data, shape):
+    """C = A op B for two CSR matrices of one shape (op: "add" / "sub" / "mul") through the two passes of
+    b2s_csr_binop_symbolic / _numeric (replaces the reference's add(), sparse/csr.py:972-1030, and mult(), :1033-1099).
+    Returns (c_indptr int64, c_indices, c_data, info), info = {nnz, a_unsorted, b_unsorted}.  When a row of A or B has
+    decreasing columns the numeric pass does not run and c_indices / c_data are None."""
+    _chk_dev(a_indptr, a_indices, a_data, b_indptr, b_indices, b_data)
+    assert a_indptr.dtype == b_indptr.dtype and a_indices.dtype == b_indices.dtype and a_data.dtype == b_data.dtype
+    a_indices, a_data, b_indices, b_data = (t.contiguous() for t in (a_indices, a_data, b_indices, b_data))
+    m, n = shape
+    dev = a_data.device
+    it, pt = idx_code(a_indices.dtype), idx_code(a_indptr.dtype)
+    st = _stream()
+    code = EW_OPS[op]
+    scratch = torch.empty(int(L.b2s_csr_binop_scratch_bytes(m)), dtype=torch.uint8, device=dev)
+    c_indptr = torch.empty(m + 1, dtype=torch.int64, device=dev)
+    out = (_lib.c_i64 * 3)()
+    _lib.check(L.b2s_csr_binop_symbolic(code, it, pt, m, n, ptr(a_indptr), ptr(a_indices), ptr(b_indptr),
+                                        ptr(b_indices), ptr(c_indptr), out, ptr(scratch), st), "b2s_csr_binop_symbolic")
+    info = {"nnz": int(out[0]), "a_unsorted": bool(out[1]), "b_unsorted": bool(out[2])}
+    if info["a_unsorted"] or info["b_unsorted"]:
+        return c_indptr, None, None, info
+    c_indices = torch.empty(info["nnz"], dtype=a_indices.dtype, device=dev)
+    c_data = torch.empty(info["nnz"], dtype=a_data.dtype, device=dev)
+    _lib.check(L.b2s_csr_binop_numeric(code, vt_code(a_data.dtype), it, pt, m, n, ptr(a_indptr), ptr(a_indices),
+                                       ptr(a_data), ptr(b_indptr), ptr(b_indices), ptr(b_data), ptr(c_indptr),
+                                       ptr(c_indices), ptr(c_data), ptr(scratch), st), "b2s_csr_binop_numeric")
+    return c_indptr, c_indices, c_data, info
+
+
+def csr_scale(indptr, indices, data, d, mode: str, shape):
+    """New values data[p] * D with A's structure through b2s_csr_scale; D (contiguous, data's dtype) holds one factor per
+    row (mode "rows"), per column ("cols") or is the row-major dense (m, n) operand ("dense")."""
+    _chk_dev(indptr, indices, data, d)
+    assert d.dtype == data.dtype and d.is_contiguous()
+    m, n = shape
+    out = torch.empty_like(data)
+    _lib.check(L.b2s_csr_scale(vt_code(data.dtype), idx_code(indices.dtype), idx_code(indptr.dtype), m, n,
+                               int(data.shape[0]), SCALE_MODES[mode], ptr(indptr), ptr(indices.contiguous()),
+                               ptr(data.contiguous()), ptr(d), n, ptr(out), _stream()), "b2s_csr_scale")
+    return out
+
+
 def spgemm_row_work(a_indptr, a_indices, b_indptr) -> torch.Tensor:
     """Products per row of A @ B (int64 device tensor of len m): the chunk planner's measure of work / output size."""
     _chk_dev(a_indptr, a_indices, b_indptr)

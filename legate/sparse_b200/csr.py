@@ -638,12 +638,138 @@ class csr_array:
     def __mul__(self, other):
         if np.isscalar(other):
             return csr_array._from_parts(self._indptr, self._indices, self._data * other, self.shape)
-        raise NotImplementedError
+        return self.multiply(other)   # elementwise, as the reference's __mul__ (csr.py:1033-1148)
 
     __rmul__ = __mul__
 
     def __neg__(self):
         return self * -1
+
+    # -- elementwise arithmetic (reference csr.py:760-776 __add__ / add, 1033-1148 mult / mult_dense) ------------------
+    def _invalidate(self):
+        """Drop the SpMV plan and every matrix derived from the arrays (after an in-place change of the structure)."""
+        self._plan = None
+        self._plan_key = None
+        for k in ("_promo_cache", "_expansion", "_transposed", "_colsplit"):
+            self.__dict__.pop(k, None)
+
+    def _binop(self, other, op: str, reverse: bool = False):
+        """self op other (other op self when `reverse`) for a sparse `other`; None when `other` is not sparse."""
+        B = _as_sparse_operand(other)
+        if B is None:
+            return None
+        if B.shape != self.shape:
+            raise ValueError(f"inconsistent shapes {self.shape} and {B.shape}")
+        A, B = cast_to_common_type(self, B)
+        if A.dtype not in SUPPORTED_VALUE_DTYPES:
+            raise NotImplementedError(f"sparse {op} for dtype {A.dtype} is not implemented (float32/float64 kernels only)")
+        return _csr_binop(B, A, op) if reverse else _csr_binop(A, B, op)
+
+    def _dense_binop(self, other, op: str, reverse: bool = False):
+        """self op other for a dense `other`: the dense result, in other's array kind (reference: todense() + other)."""
+        common = np.result_type(self.dtype, numpy_dtype(other.dtype))
+        if common.kind == "c":
+            raise NotImplementedError("complex elementwise operations are not implemented")
+        if isinstance(other, torch.Tensor):
+            D = torch.zeros(self.shape, dtype=torch_dtype(common), device=other.device)
+            counts = (self._indptr[1:] - self._indptr[:-1]).to(torch.int64)
+            rows = torch.repeat_interleave(torch.arange(self.shape[0], dtype=torch.int64, device=self.device), counts)
+            D.index_put_((rows.to(other.device), self._indices.to(device=other.device, dtype=torch.int64)),
+                         self._data.to(device=other.device, dtype=D.dtype), accumulate=True)
+        else:
+            D = self.todense().astype(common, copy=False)
+        if op == "add":
+            return D + other
+        return other - D if reverse else D - other
+
+    def _scalar_binop(self, other, op: str, reverse: bool = False):
+        if other != 0:
+            raise NotImplementedError(f"{'adding' if op == 'add' else 'subtracting'} a nonzero scalar to a sparse matrix "
+                                      "is not supported")
+        return -self if (reverse and op == "sub") else self.copy()
+
+    def _arith(self, other, op: str, reverse: bool = False):
+        if np.isscalar(other):
+            return self._scalar_binop(other, op, reverse)
+        C = self._binop(other, op, reverse)
+        if C is not None:
+            return C
+        if isinstance(other, (np.ndarray, torch.Tensor)):
+            return self._dense_binop(other, op, reverse)
+        return NotImplemented
+
+    def __add__(self, other):
+        return self._arith(other, "add")
+
+    def __radd__(self, other):
+        return self._arith(other, "add", reverse=True)
+
+    def __sub__(self, other):
+        return self._arith(other, "sub")
+
+    def __rsub__(self, other):
+        return self._arith(other, "sub", reverse=True)
+
+    def multiply(self, other):
+        """Elementwise product.  Sparse `other`: the intersection of the two structures.  Dense `other` of shape (m, n),
+        (m, 1), (1, n) or (n,): A's structure, each value times its entry of `other` (broadcast along rows / columns)."""
+        if np.isscalar(other):
+            return self * other
+        C = self._binop(other, "mul")
+        if C is not None:
+            return C
+        D = other if isinstance(other, torch.Tensor) else np.asarray(other)
+        if D.ndim == 0:
+            return self * D.item()
+        m, n = self.shape
+        shape = tuple(D.shape)
+        if shape == (m, n):
+            mode = "dense"
+        elif shape == (m, 1):
+            mode = "rows"
+        elif shape in ((1, n), (n,)):
+            mode = "cols"
+        else:
+            raise ValueError(f"inconsistent shapes {self.shape} and {shape}")
+        common = np.result_type(self.dtype, numpy_dtype(D.dtype))
+        if common not in SUPPORTED_VALUE_DTYPES:
+            raise NotImplementedError(f"multiply for dtype {common} is not implemented (float32/float64 kernels only)")
+        runtime.require_cuda("csr_array.multiply")
+        A = self.astype(common, copy=False)
+        Dd = to_device(D, dtype=common).reshape(-1)
+        data = _ops.csr_scale(A._indptr, A._indices, A._data, Dd, mode, self.shape)
+        return csr_array._from_parts(A._indptr, A._indices, data, self.shape)
+
+    def eliminate_zeros(self):
+        """Remove the explicitly stored zeros (either sign), in place."""
+        keep = self._data != 0
+        if bool(keep.all()):
+            return
+        kept = torch.zeros(self.nnz + 1, dtype=torch.int64, device=keep.device)
+        torch.cumsum(keep.to(torch.int64), 0, out=kept[1:])
+        self._indptr = kept[self._indptr.to(torch.int64)].to(self._indptr.dtype)
+        self._indices = self._indices[keep]
+        self._data = self._data[keep]
+        self._invalidate()
+
+    @property
+    def has_sorted_indices(self) -> bool:
+        """True when the columns of every row are non-decreasing."""
+        nnz = self.nnz
+        if nnz < 2:
+            return True
+        drop = self._indices[1:] < self._indices[:-1]
+        starts = self._indptr[1:-1].to(torch.int64)
+        starts = starts[(starts > 0) & (starts < nnz)]
+        drop[starts - 1] = False        # the first entry of a row is not compared with the previous row's last
+        return not bool(drop.any())
+
+    def sort_indices(self):
+        """Sort the columns of every row, in place (new index / value arrays: other matrices sharing them keep theirs)."""
+        if self.has_sorted_indices:
+            return
+        self._indices, self._data = _ops.csr_sort_rows(self._indptr, self._indices.clone(), self._data.clone())
+        self._invalidate()
 
     def balance(self):
         """No-op on a single device; kept for API parity (reference base.py:198-282 re-tiles the rows by
@@ -680,6 +806,48 @@ def spgemm_csr_csr_csr(A: csr_array, B: csr_array) -> csr_array:
     C = csr_array._from_parts(c_ptr, c_idx, c_val, (A.shape[0], B.shape[1]))
     C.spgemm_info = info
     return C
+
+
+def _as_sparse_operand(other):
+    """`other` as a csr_array when it is a sparse matrix (csr_array, coo_array, what diags() returns, scipy.sparse),
+    else None."""
+    if isinstance(other, csr_array):
+        return other
+    if scipy.sparse.issparse(other):
+        return csr_array(other)
+    if hasattr(other, "tocsr") and not isinstance(other, (np.ndarray, torch.Tensor)):
+        csr = other.tocsr()
+        if isinstance(csr, csr_array):
+            return csr
+    return None
+
+
+def _csr_binop(A: csr_array, B: csr_array, op: str) -> csr_array:
+    """C = A op B (op "add" / "sub" / "mul") for operands of one shape and dtype: the row merge of csrc/elementwise.cu.
+    Operands with a decreasing row are merged from sorted copies; their own arrays are left as they are."""
+    runtime.require_cuda(f"csr_array {op}")
+    a_ptr, b_ptr, a_idx, b_idx = A._indptr, B._indptr, A._indices, B._indices
+    if a_ptr.dtype != b_ptr.dtype:
+        a_ptr, b_ptr = a_ptr.to(torch.int64), b_ptr.to(torch.int64)
+    if a_idx.dtype != b_idx.dtype:
+        a_idx, b_idx = a_idx.to(torch.int64), b_idx.to(torch.int64)
+    a_val, b_val = A._data, B._data
+    c_ptr, c_idx, c_val, info = _ops.csr_binop(op, a_ptr, a_idx, a_val, b_ptr, b_idx, b_val, A.shape)
+    if c_idx is None:
+        if info["a_unsorted"]:
+            a_idx, a_val = _ops.csr_sort_rows(a_ptr, a_idx.clone(), a_val.clone())
+        if info["b_unsorted"]:
+            b_idx, b_val = _ops.csr_sort_rows(b_ptr, b_idx.clone(), b_val.clone())
+        c_ptr, c_idx, c_val, info = _ops.csr_binop(op, a_ptr, a_idx, a_val, b_ptr, b_idx, b_val, A.shape)
+        assert c_idx is not None, "row sort left a decreasing row"
+    wide = _force_wide()
+    if info["nnz"] <= _INT32_MAX and not wide:
+        c_ptr = c_ptr.to(torch.int32)
+    if wide:
+        c_idx = c_idx.to(torch.int64)
+    elif c_idx.dtype == torch.int64 and A.shape[1] - 1 <= _INT32_MAX:
+        c_idx = c_idx.to(torch.int32)
+    return csr_array._from_parts(c_ptr, c_idx, c_val, A.shape)
 
 
 def spgemm_chunked(A: csr_array, B: csr_array, max_products: int = 1 << 31, keep: bool = False, on_chunk=None):

@@ -16,11 +16,10 @@
 // entry recovered from indptr (binary search), replacing the argsort the Python layer used before.
 // HBM/L2-atomic-bound integer work: ~nnz*(2*si + sv) read + the same written, twice.
 #include "common.cuh"
+#include "scan.cuh"
 #include <algorithm>
 
 namespace b2s {
-
-constexpr int CV_SCAN_BLOCK = 1024;
 
 template <typename T> __device__ __forceinline__ T cv_atomic_inc(T* p);
 template <> __device__ __forceinline__ int32_t cv_atomic_inc<int32_t>(int32_t* p) { return atomicAdd(p, 1); }
@@ -49,59 +48,6 @@ cv_count_kernel(int64_t nnz, const I* __restrict__ keys, P* __restrict__ cnt, in
     if (b < 0 || b >= nbuckets) { atomicAdd(bad, 1ull); continue; }
     cv_atomic_inc<P>(cnt + b + 1);   // cnt[b+1]: the scan below then yields indptr directly
   }
-}
-
-template <typename P>
-__global__ void __launch_bounds__(256) cv_scan_block_kernel(int64_t n, P* __restrict__ data, long long* __restrict__ block_sums) {
-  // inclusive scan of data[0..n) in blocks of CV_SCAN_BLOCK; block totals to block_sums
-  __shared__ long long warp_tot[8];
-  const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-  const int64_t base = (int64_t)blockIdx.x * CV_SCAN_BLOCK + tid * 4;
-  long long v[4];
-#pragma unroll
-  for (int q = 0; q < 4; q++) v[q] = (base + q < n) ? (long long)data[base + q] : 0;
-  v[1] += v[0]; v[2] += v[1]; v[3] += v[2];
-  long long inc = v[3];
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) { const long long t = __shfl_up_sync(0xffffffffu, inc, o); if (lane >= o) inc += t; }
-  if (lane == 31) warp_tot[wid] = inc;
-  __syncthreads();
-  long long woff = 0, tot = 0;
-  for (int w = 0; w < 8; w++) { if (w < wid) woff += warp_tot[w]; tot += warp_tot[w]; }
-  const long long excl = woff + inc - v[3];
-#pragma unroll
-  for (int q = 0; q < 4; q++) if (base + q < n) data[base + q] = (P)(excl + v[q]);
-  if (tid == 0) block_sums[blockIdx.x] = tot;
-}
-__global__ void __launch_bounds__(1024) cv_scan_sums_kernel(int64_t nblocks, long long* __restrict__ block_sums) {
-  // exclusive scan of the block totals by one CTA (sequential over chunks of 1024)
-  __shared__ long long s[1024];
-  __shared__ long long carry;
-  if (threadIdx.x == 0) carry = 0;
-  __syncthreads();
-  for (int64_t c0 = 0; c0 < nblocks; c0 += 1024) {
-    const int64_t i = c0 + threadIdx.x;
-    const long long v = i < nblocks ? block_sums[i] : 0;
-    s[threadIdx.x] = v;
-    __syncthreads();
-    for (int o = 1; o < 1024; o <<= 1) {
-      const long long t = threadIdx.x >= o ? s[threadIdx.x - o] : 0;
-      __syncthreads();
-      s[threadIdx.x] += t;
-      __syncthreads();
-    }
-    if (i < nblocks) block_sums[i] = carry + s[threadIdx.x] - v;
-    __syncthreads();
-    if (threadIdx.x == 0) carry += s[1023];
-    __syncthreads();
-  }
-}
-template <typename P>
-__global__ void __launch_bounds__(256) cv_scan_add_kernel(int64_t n, P* __restrict__ data, const long long* __restrict__ block_sums) {
-  const int64_t i = (int64_t)blockIdx.x * CV_SCAN_BLOCK + threadIdx.x * 4;
-  const long long add = block_sums[blockIdx.x];
-#pragma unroll
-  for (int q = 0; q < 4; q++) if (i + q < n) data[i + q] = (P)((long long)data[i + q] + add);
 }
 
 // fill: COO flavour (explicit rows) and transpose flavour (bucket = column, payload = row id found from indptr)
@@ -243,6 +189,37 @@ static CvScratch cv_layout(int64_t nbuckets, int pbytes) {
   return L;
 }
 
+// sort every row of (indptr, idx, val) by column: the warp kernel takes rows of <= 32 entries, the longer ones are
+// listed and sorted one CTA per row.  counters[0..1] (bad keys, long rows) must be zeroed on the stream; syncs once to
+// read them back (*bad_host = counters[0]).
+template <typename V, typename I, typename P>
+static int cv_sort_rows(const DeviceProps& pr, int64_t nrows, int64_t nnz, const P* indptr, I* idx, V* val,
+                        unsigned long long* counters, int64_t* list, int64_t* bad_host, cudaStream_t st) {
+  if (nnz > 0) {
+    const unsigned gb = (unsigned)std::min<int64_t>((nrows + 1 + 255) / 256, (int64_t)pr.sm_count * 16);
+    const unsigned gw = (unsigned)std::min<int64_t>((nrows * 32 + 255) / 256, (int64_t)pr.sm_count * 32);
+    cv_sort_warp_kernel<V, I, P><<<gw ? gw : 1, 256, 0, st>>>(nrows, indptr, idx, val);
+    B2S_LAUNCH_CHECK();
+    cv_long_rows_kernel<P><<<gb, 256, 0, st>>>(nrows, indptr, list, counters + 1);
+    B2S_LAUNCH_CHECK();
+  }
+  unsigned long long host_counters[2] = {0, 0};
+  B2S_CUDA(cudaMemcpyAsync(host_counters, counters, sizeof(host_counters), cudaMemcpyDeviceToHost, st));
+  B2S_CUDA(cudaStreamSynchronize(st));
+  if (bad_host) *bad_host = (int64_t)host_counters[0];
+  if (host_counters[1] > 0) {
+    constexpr int CAP = 4096;
+    auto kern = cv_sort_cta_kernel<V, I, P, CAP>;
+    const size_t smem = (sizeof(I) + sizeof(V)) * CAP;
+    struct TagSort {};
+    if (int rc = ensure_dyn_smem<TagSort>(kern, (int)smem)) return rc;
+    const unsigned gl = (unsigned)std::min<int64_t>((int64_t)host_counters[1], (int64_t)pr.sm_count * 4);
+    kern<<<gl, 256, smem, st>>>((int64_t)host_counters[1], list, indptr, idx, val);
+    B2S_LAUNCH_CHECK();
+  }
+  return B2S_OK;
+}
+
 template <typename V, typename I, typename P, typename PIN, bool TRANSPOSE>
 static int cv_run(int64_t nbuckets, int64_t nnz, const I* rows, const I* cols, const V* vals, const PIN* in_indptr,
                   int64_t in_nrows, P* indptr, I* out_idx, V* out_val, unsigned char* scratch, int64_t* bad_host,
@@ -262,13 +239,7 @@ static int cv_run(int64_t nbuckets, int64_t nnz, const I* rows, const I* cols, c
     B2S_LAUNCH_CHECK();
   }
   const int64_t n1 = nbuckets + 1;
-  const int64_t nblocks = (n1 + CV_SCAN_BLOCK - 1) / CV_SCAN_BLOCK;
-  cv_scan_block_kernel<P><<<(unsigned)nblocks, 256, 0, st>>>(n1, indptr, sums);
-  B2S_LAUNCH_CHECK();
-  cv_scan_sums_kernel<<<1, 1024, 0, st>>>(nblocks, sums);
-  B2S_LAUNCH_CHECK();
-  cv_scan_add_kernel<P><<<(unsigned)nblocks, 256, 0, st>>>(n1, indptr, sums);
-  B2S_LAUNCH_CHECK();
+  if (int rc = cv_inclusive_scan<P>(indptr, n1, sums, st)) return rc;
   const unsigned gb = (unsigned)std::min<int64_t>((n1 + 255) / 256, (int64_t)pr.sm_count * 16);
   cv_copy_cursor_kernel<P><<<gb, 256, 0, st>>>(n1, indptr, cursor);
   B2S_LAUNCH_CHECK();
@@ -276,27 +247,8 @@ static int cv_run(int64_t nbuckets, int64_t nnz, const I* rows, const I* cols, c
     cv_fill_kernel<V, I, P, PIN, TRANSPOSE><<<gn ? gn : 1, 256, 0, st>>>(nnz, rows, cols, vals, in_indptr, in_nrows, nbuckets,
                                                                          cursor, out_idx, out_val);
     B2S_LAUNCH_CHECK();
-    const unsigned gw = (unsigned)std::min<int64_t>((nbuckets * 32 + 255) / 256, (int64_t)pr.sm_count * 32);
-    cv_sort_warp_kernel<V, I, P><<<gw ? gw : 1, 256, 0, st>>>(nbuckets, indptr, out_idx, out_val);
-    B2S_LAUNCH_CHECK();
-    cv_long_rows_kernel<P><<<gb, 256, 0, st>>>(nbuckets, indptr, list, counters + 1);
-    B2S_LAUNCH_CHECK();
   }
-  unsigned long long host_counters[2] = {0, 0};
-  B2S_CUDA(cudaMemcpyAsync(host_counters, counters, sizeof(host_counters), cudaMemcpyDeviceToHost, st));
-  B2S_CUDA(cudaStreamSynchronize(st));
-  if (bad_host) *bad_host = (int64_t)host_counters[0];
-  if (host_counters[1] > 0) {
-    constexpr int CAP = 4096;
-    auto kern = cv_sort_cta_kernel<V, I, P, CAP>;
-    const size_t smem = (sizeof(I) + sizeof(V)) * CAP;
-    struct TagSort {};
-    if (int rc = ensure_dyn_smem<TagSort>(kern, (int)smem)) return rc;
-    const unsigned gl = (unsigned)std::min<int64_t>((int64_t)host_counters[1], (int64_t)pr.sm_count * 4);
-    kern<<<gl, 256, smem, st>>>((int64_t)host_counters[1], list, indptr, out_idx, out_val);
-    B2S_LAUNCH_CHECK();
-  }
-  return B2S_OK;
+  return cv_sort_rows<V, I, P>(pr, nbuckets, nnz, indptr, out_idx, out_val, counters, list, bad_host, st);
 }
 
 }  // namespace b2s
@@ -365,6 +317,37 @@ int b2s_csr_transpose(int vt, int it, int pt, int64_t nrows, int64_t ncols, int6
 #undef B2S_CT
   B2S_CHECK_ARG(bad == 0, "%lld column indices outside [0, ncols)", (long long)bad);
   return B2S_OK;
+}
+
+/* Sort every row of a CSR matrix by column, in place (the row sort of the two calls above).  Rows with repeated
+ * columns keep them adjacent, in unspecified order.  `scratch`: b2s_convert_scratch_bytes(nrows, pt) bytes.  Syncs
+ * the stream once. */
+int b2s_csr_sort_rows(int vt, int it, int pt, int64_t nrows, int64_t nnz, const void* indptr, void* indices,
+                      void* vals, void* scratch, void* stream) {
+  B2S_CHECK_ARG(vt == B2S_F32 || vt == B2S_F64, "bad value type code %d", vt);
+  B2S_CHECK_ARG((it == B2S_I32 || it == B2S_I64) && (pt == B2S_I32 || pt == B2S_I64), "bad index type codes");
+  B2S_CHECK_ARG(nrows >= 0 && nnz >= 0 && indptr && scratch, "bad arguments");
+  B2S_CHECK_ARG(nnz == 0 || (indices && vals), "NULL array with nnz > 0");
+  DeviceProps pr;
+  if (int rc = get_props(&pr)) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  unsigned char* sc = (unsigned char*)scratch;
+  const CvScratch L = cv_layout(nrows, pt == B2S_I64 ? 8 : 4);
+  unsigned long long* counters = (unsigned long long*)(sc + L.off_counters);
+  int64_t* list = (int64_t*)(sc + L.off_list);
+  B2S_CUDA(cudaMemsetAsync(counters, 0, 256, st));
+#define B2S_SR(V, I, P) return cv_sort_rows<V, I, P>(pr, nrows, nnz, (const P*)indptr, (I*)indices, (V*)vals, counters, list, nullptr, st)
+  switch ((vt == B2S_F64 ? 4 : 0) + (it == B2S_I64 ? 2 : 0) + (pt == B2S_I64 ? 1 : 0)) {
+    case 0: B2S_SR(float, int32_t, int32_t);
+    case 1: B2S_SR(float, int32_t, int64_t);
+    case 2: B2S_SR(float, int64_t, int32_t);
+    case 3: B2S_SR(float, int64_t, int64_t);
+    case 4: B2S_SR(double, int32_t, int32_t);
+    case 5: B2S_SR(double, int32_t, int64_t);
+    case 6: B2S_SR(double, int64_t, int32_t);
+    default: B2S_SR(double, int64_t, int64_t);
+  }
+#undef B2S_SR
 }
 
 }  // extern "C"
