@@ -73,7 +73,8 @@ int64_t     b2s_ws_bytes(void);
  *   b2s_spmv_plan_destroy: frees the host handle (never the device buffer).
  *   b2s_spmv_plan_info  : out[0]=tile config id, out[1]=bit0 row-group kernel, bit1 uniform-row path, bit2 scattered, bit3 short-row
  *                         (one lane per row) path, bit4 TMA tile kind, bit5 packed structure, bit6 coded values,
- *                         bits 8..12 distinct values of a coded plan, out[2]=tiles,
+ *                         bit7 row templates, bits 8..12 distinct values of a coded plan, bits 16..23 row templates
+ *                         of the plan, out[2]=tiles,
  *                         out[3]=1000*lines-per-warp statistic. */
 int64_t     b2s_spmv_plan_tiles(int vt, int64_t nrows, int64_t nnz);
 int64_t     b2s_spmv_plan_bytes(int vt, int64_t nrows, int64_t nnz);
@@ -105,12 +106,30 @@ int         b2s_spmv_plan_info(const void* plan, int64_t* out4_host);
  *                             theirs.  An edit of vals afterwards (even in place) needs a new plan; otherwise it packs
  *                             exactly as b2s_spmv_plan_pack;
  *   b2s_spmv_plan_set_packed: 0 = launches read indptr / indices again, 1 = the packed form with streamed values,
- *                             2 = the packed form with coded values (tests / tools). */
+ *                             2 = the packed form with coded values, 3 = row templates (below) for b2s_spmv_csr /
+ *                             _dot and the coded, else packed, else CSR form for every other launch (tests / tools).
+ *
+ * Row templates.  The signature of a row is its length, then column - row of each entry in stored order, then the bit
+ * patterns of the values.  When every row has at most 8 entries and the matrix has at most 32 distinct signatures
+ * (stencils on structured grids: 9 for a 5-point Laplacian, 27 for a 3-D 7-point one), the plan can hold the distinct
+ * signatures and one uint8 template id per row; b2s_spmv_csr and b2s_spmv_csr_dot with the same `vals` pointer then
+ * read the ids, x and y only, and compute y bit for bit as the other kernels of the plan do.  The tile-range, fused,
+ * accumulating and host-vector entry points keep the tile kernels.
+ *   b2s_spmv_plan_templates_bytes: size of the DEVICE buffer (16-byte aligned) they need; 0 = the plan cannot use them
+ *                                  (only plans whose tiles all take the one-lane-per-row kernel can);
+ *   b2s_spmv_plan_templates      : detects the templates (two passes over the matrix, every row compared with its
+ *                                  template entry by entry; two host syncs) and, when the matrix qualifies, writes them
+ *                                  to the buffer, which must then outlive every launch with the plan; an edit of
+ *                                  indptr, indices or vals afterwards needs a new plan.  A matrix that does not
+ *                                  qualify leaves the plan as it was.  b2s_spmv_plan_info reports the outcome. */
 int64_t     b2s_spmv_plan_pack_bytes(const void* plan);
 int         b2s_spmv_plan_pack(void* plan, const void* indptr, const void* indices, void* pack_buf_dev, void* stream);
 int         b2s_spmv_plan_pack_coded(void* plan, const void* indptr, const void* indices, const void* vals,
                                      void* pack_buf_dev, void* stream);
 int         b2s_spmv_plan_set_packed(void* plan, int mode);
+int64_t     b2s_spmv_plan_templates_bytes(const void* plan);
+int         b2s_spmv_plan_templates(void* plan, const void* indptr, const void* indices, const void* vals,
+                                    void* tpl_buf_dev, void* stream);
 
 /* y = A x  (alpha=1, beta=0 as spmv.cu:79-80).  `plan` may be NULL: then a plan-free
  * row-per-lane-group kernel is used (slower on short rows).  `plan` is the HOST handle

@@ -37,6 +37,8 @@ SIGNATURES = {
     "b2s_spmv_plan_pack": (c_i32, [c_vp, c_vp, c_vp, c_vp, c_vp]),
     "b2s_spmv_plan_pack_coded": (c_i32, [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "b2s_spmv_plan_set_packed": (c_i32, [c_vp, c_i32]),
+    "b2s_spmv_plan_templates_bytes": (c_i64, [c_vp]),
+    "b2s_spmv_plan_templates": (c_i32, [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "b2s_spmv_csr": (c_i32, [c_i32, c_i32, c_i32, c_i64, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "b2s_spmm_csr": (c_i32, [c_i32, c_i32, c_i32, c_i64, c_i64, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp,
                              c_i64, c_vp]),
@@ -100,6 +102,7 @@ SIGNATURES = {
     "b2s_spmv_num_configs": (c_i32, []),
     "b2s_spmv_plan_set_kernel": (c_i32, [c_vp, c_i32]),
     "b2s_spmv_plan_set_flavor": (c_i32, [c_vp, c_i32]),
+    "b2s_spmv_set_template_config": (c_i32, [c_i32, c_i32, c_i32]),
 }
 
 

@@ -38,6 +38,8 @@ class SpmvPlan:
         # the packed structure (b2s_spmv_plan_pack / _pack_coded), read by every launch with this plan: it lives as long
         # as the plan, and is never rewritten (a captured launch may still read it)
         self.pack_buf = pack_buf
+        # the row templates (b2s_spmv_plan_templates): same lifetime rule as pack_buf
+        self.tpl_buf = None
         self._info()
 
     def _info(self):
@@ -46,6 +48,7 @@ class SpmvPlan:
         self.config, self.rowgroup, self.uniform, self.scattered = int(out[0]), bool(out[1] & 1), bool(out[1] & 2), bool(out[1] & 4)
         self.short_rows, self.tma, self.packed = bool(out[1] & 8), bool(out[1] & 16), bool(out[1] & 32)
         self.coded, self.ndict = bool(out[1] & 64), int(out[1] >> 8) & 31
+        self.templated, self.ntemplates = bool(out[1] & 128), int(out[1] >> 16) & 255
         self.tiles, self.lines_per_warp = int(out[2]), out[3] / 1000.0
 
     @property
@@ -70,7 +73,8 @@ class SpmvPlan:
 
     def set_packed(self, mode):
         """tools / tests: 0 / False = stream the CSR arrays, 1 / True = the packed structure and the values, 2 = the
-        packed structure with coded values (the plan must have been packed / coded)."""
+        packed structure with coded values (the plan must have been packed / coded), 3 = row templates for whole-matrix
+        products (the plan must have them)."""
         _lib.check(L.b2s_spmv_plan_set_packed(self.handle, int(mode)), "b2s_spmv_plan_set_packed")
         self._info()
 
@@ -84,7 +88,11 @@ class SpmvPlan:
             fl += ", packed u16 columns/row offsets"
         if self.coded:
             fl += f", coded values ({self.ndict} distinct)"
-        return f"b2s::spmv_{'tma' if self.tma else 'tile'}_kernel cfg {self.config} [{fl}]"
+        tiles = f"b2s::spmv_{'tma' if self.tma else 'tile'}_kernel cfg {self.config} [{fl}]"
+        if self.templated:
+            # whole-matrix products; tile ranges, fused exchanges and y += A x keep the tile kernel
+            return f"b2s::spmv_template_kernel [{self.ntemplates} row templates, uint8 id per row; tiles: {tiles}]"
+        return tiles
 
     def __del__(self):
         h, self.handle = getattr(self, "handle", None), None
@@ -141,6 +149,27 @@ def spmv_plan_code(plan: SpmvPlan, indptr: torch.Tensor, indices: torch.Tensor, 
     _lib.check(L.b2s_spmv_plan_pack_coded(plan.handle, ptr(indptr), ptr(indices), ptr(data), ptr(plan.pack_buf),
                                           _stream()), "b2s_spmv_plan_pack_coded")
     plan._info()
+    return plan
+
+
+def spmv_plan_templates(plan: SpmvPlan, indptr: torch.Tensor, indices: torch.Tensor, data: torch.Tensor) -> SpmvPlan:
+    """Give a plan that no launch has used yet row templates when the matrix qualifies (rows of at most 8 entries, at
+    most 32 distinct (length, column - row, value bits) signatures -- structured-grid stencils): whole-matrix products
+    with this `data` then read one uint8 id per row instead of the matrix, so the plan is also only valid while `data`
+    is unchanged.  Otherwise, or for a plan that cannot use them, the plan is returned as it was."""
+    if getattr(plan, "handle", None) is None:
+        return plan
+    nbytes = int(L.b2s_spmv_plan_templates_bytes(plan.handle))
+    if nbytes <= 0:
+        return plan
+    _chk_dev(data)
+    assert data.is_contiguous() and data.shape[0] == plan.nnz
+    buf = torch.empty(nbytes // 4, dtype=torch.int32, device=indptr.device)
+    _lib.check(L.b2s_spmv_plan_templates(plan.handle, ptr(indptr), ptr(indices), ptr(data), ptr(buf), _stream()),
+               "b2s_spmv_plan_templates")
+    plan._info()
+    if plan.ntemplates:
+        plan.tpl_buf = buf
     return plan
 
 

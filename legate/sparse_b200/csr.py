@@ -285,6 +285,7 @@ class csr_array:
             plan = _ops.spmv_plan(self._indptr, self._indices, self.shape, self.nnz, self.dtype, tma_only=tma_only)
             if self._data.is_contiguous():
                 plan = _ops.spmv_plan_code(plan, self._indptr, self._indices, self._data)
+                plan = _ops.spmv_plan_templates(plan, self._indptr, self._indices, self._data)
             self._plan = plan
             self._plan_key = key
         return self._plan

@@ -14,6 +14,8 @@ namespace b2s {
 // tuning hooks (tools/, tests): -1 / 0 = automatic
 static std::atomic<int> g_cfg{-1};
 static std::atomic<int> g_waves{0};
+// row-template kernel shape (tools / tests): rows per lane, threads per CTA, evict-first y stores; 0 = default
+static std::atomic<int> g_tpl_rows{0}, g_tpl_threads{0}, g_tpl_streaming{0};
 
 static inline int resolve_cfg(int vt, bool scattered, bool likely_short) {
   const int forced = g_cfg.load();
@@ -290,6 +292,148 @@ spmv_dict_kernel(const U* __restrict__ vals, int64_t n, unsigned long long* __re
   if (threadIdx.x == 0) counts[blockIdx.x] = cnt;
 }
 
+// ---- row templates (TemplateTable) ------------------------------------------------------------------------------
+__device__ __forceinline__ unsigned long long tpl_mix(unsigned long long h, unsigned long long v) {
+  h ^= v + 0x9e3779b97f4a7c15ull + (h << 6) + (h >> 2);
+  h *= 0xff51afd7ed558ccdull;
+  return h ^ (h >> 33);
+}
+__device__ __forceinline__ unsigned long long tpl_bits(const void* vals, int vbytes, long long k) {
+  return vbytes == 8 ? reinterpret_cast<const unsigned long long*>(vals)[k]
+                     : (unsigned long long)reinterpret_cast<const unsigned*>(vals)[k];
+}
+// Hash of row r's signature (length, column - r, value bits); false when the row cannot be a template (longer than
+// kTplLen, or an offset outside int32).  The hash is only a lookup key: tpl_assign_kernel compares every entry.
+template <typename I, typename P>
+__device__ __forceinline__ bool tpl_row_hash(const P* __restrict__ indptr, const I* __restrict__ indices,
+                                             const void* __restrict__ vals, int vbytes, long long r,
+                                             unsigned long long* hash) {
+  const long long k0 = (long long)indptr[r], n = (long long)indptr[r + 1] - k0;
+  if (n < 0 || n > kTplLen) return false;
+  unsigned long long h = tpl_mix(0, (unsigned long long)n);
+  for (int j = 0; j < (int)n; j++) {
+    const long long d = (long long)indices[k0 + j] - r;
+    if (d < INT_MIN || d > INT_MAX) return false;
+    h = tpl_mix(tpl_mix(h, (unsigned long long)(unsigned)(int)d), tpl_bits(vals, vbytes, k0 + j));
+  }
+  *hash = h;
+  return true;
+}
+
+// Pass 1: the distinct signature hashes of the rows, per block, with one representative row each -- modelled on
+// spmv_dict_kernel (a bounded shared table, misses inserted under a block lock).  counts[block] > kMaxTemplates: the
+// block saw more signatures than that, or a row that cannot be a template.
+constexpr int kTplBlocks = 1024;
+template <typename I, typename P>
+__global__ void __launch_bounds__(256)
+tpl_collect_kernel(int64_t nrows, const P* __restrict__ indptr, const I* __restrict__ indices,
+                   const void* __restrict__ vals, int vbytes, unsigned long long* __restrict__ tabs,
+                   long long* __restrict__ reps, int* __restrict__ counts) {
+  constexpr int CAP = kMaxTemplates + 1;
+  __shared__ unsigned long long th[CAP];
+  __shared__ long long tr[CAP];
+  __shared__ int cnt, lock, bad;
+  if (threadIdx.x == 0) { cnt = 0; lock = 0; bad = 0; }
+  __syncthreads();
+  volatile unsigned long long* vth = th;
+  volatile long long* vtr = tr;
+  volatile int* vcnt = &cnt;
+  volatile int* vbad = &bad;
+  const unsigned full = 0xffffffffu;
+  const int lane = threadIdx.x & 31;
+  const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+  for (int64_t base = warp * 32; base < nrows; base += nwarps * 32) {      // warp-uniform
+    if (__shfl_sync(full, (*vcnt > kMaxTemplates || *vbad) ? 1 : 0, 0)) break;
+    const long long r = base + lane;
+    unsigned long long h = 0;
+    bool in = r < nrows;
+    if (in && !tpl_row_hash(indptr, indices, vals, vbytes, r, &h)) { *vbad = 1; in = false; }
+    const int c = *vcnt;
+    bool hit = !in;
+    for (int i = 0; i < c && i < CAP && !hit; i++) hit = vth[i] == h;
+    unsigned miss = __ballot_sync(full, !hit);
+    if (!miss) continue;
+    if (lane == 0) while (atomicCAS(&lock, 0, 1) != 0) {}
+    __syncwarp();
+    __threadfence_block();
+    while (miss) {
+      const int src = __ffs(miss) - 1;
+      const unsigned long long cand = __shfl_sync(full, h, src);
+      const long long crow = __shfl_sync(full, r, src);
+      const int c2 = *vcnt;
+      bool found = false;
+      for (int i = 0; i < c2 && i < CAP; i++) found = found || vth[i] == cand;
+      if (lane == 0 && !found && c2 < CAP) {
+        vth[c2] = cand;
+        vtr[c2] = crow;
+        __threadfence_block();
+        *vcnt = c2 + 1;
+      }
+      __syncwarp();
+      miss &= ~__ballot_sync(full, in && h == cand);
+    }
+    __threadfence_block();
+    __syncwarp();
+    if (lane == 0) atomicExch(&lock, 0);
+  }
+  __syncthreads();
+  const int c = cnt < CAP ? cnt : CAP;
+  if ((int)threadIdx.x < c) {
+    tabs[(int64_t)blockIdx.x * CAP + threadIdx.x] = th[threadIdx.x];
+    reps[(int64_t)blockIdx.x * CAP + threadIdx.x] = tr[threadIdx.x];
+  }
+  if (threadIdx.x == 0) counts[blockIdx.x] = bad ? CAP + 1 : cnt;
+}
+
+// The table from the representative rows reps[0, n) (one thread per template; hashes ascending)
+template <typename I, typename P>
+__global__ void tpl_table_kernel(const P* __restrict__ indptr, const I* __restrict__ indices,
+                                 const void* __restrict__ vals, int vbytes, const long long* __restrict__ reps, int n,
+                                 TemplateTable* __restrict__ tab) {
+  const int t = threadIdx.x;
+  if (t >= n) return;
+  const long long r = reps[t];
+  const long long k0 = (long long)indptr[r];
+  const int len = (int)((long long)indptr[r + 1] - k0);
+  unsigned long long h = 0;
+  tpl_row_hash(indptr, indices, vals, vbytes, r, &h);
+  tab->hash[t] = h;
+  tab->len[t] = len;
+  for (int j = 0; j < kTplLen; j++) {
+    tab->off[t][j] = j < len ? (int)((long long)indices[k0 + j] - r) : 0;
+    tab->bits[t][j] = j < len ? tpl_bits(vals, vbytes, k0 + j) : 0ull;
+  }
+}
+
+// Pass 2: ids[r] = the template whose hash matches row r's, after comparing the row with it entry by entry; any row
+// that matches no template sets *bad (a hash collision among them included), and the plan then has no templates.
+template <typename I, typename P>
+__global__ void __launch_bounds__(256)
+tpl_assign_kernel(int64_t nrows, const P* __restrict__ indptr, const I* __restrict__ indices,
+                  const void* __restrict__ vals, int vbytes, const TemplateTable* __restrict__ tab, int n,
+                  uint8_t* __restrict__ ids, int* __restrict__ bad) {
+  __shared__ unsigned long long sh[kMaxTemplates];
+  if ((int)threadIdx.x < kMaxTemplates) sh[threadIdx.x] = tab->hash[threadIdx.x];
+  __syncthreads();
+  const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= nrows) return;
+  unsigned long long h = 0;
+  int t = -1;
+  if (tpl_row_hash(indptr, indices, vals, vbytes, r, &h))
+    for (int i = 0; i < n; i++) t = sh[i] == h ? i : t;
+  bool ok = t >= 0;
+  if (ok) {
+    const long long k0 = (long long)indptr[r];
+    const int len = (int)((long long)indptr[r + 1] - k0);
+    ok = len == tab->len[t];
+    for (int j = 0; ok && j < len; j++)
+      ok = (long long)indices[k0 + j] - r == (long long)tab->off[t][j] && tpl_bits(vals, vbytes, k0 + j) == tab->bits[t][j];
+  }
+  ids[r] = (uint8_t)(ok ? t : 0);
+  if (!ok) atomicExch(bad, 1);
+}
+
 // Sections of the packed-structure buffer: tile bases, columns, row offsets, value dictionary (each 16-byte aligned)
 static inline int64_t round16(int64_t b) { return (b + 15) & ~(int64_t)15; }
 constexpr int64_t kDictBytes = kMaxDict * 8;
@@ -319,6 +463,11 @@ struct PlanHandle {
   PackedTiles pk;   // the packed structure in the caller's buffer (NULL until packed; dict NULL unless coded)
   const void* coded_vals;               // the values the codes were built from
   unsigned char dict_img[kDictBytes];   // host copy of the dictionary written to the buffer
+  // row templates (b2s_spmv_plan_templates): the table + ids in the caller's buffer (NULL until built), the values they
+  // were built from, the number of templates and the longest; use_tpl: whole-matrix launches with tpl_vals run them
+  const TemplateTable* tpl;
+  const void* tpl_vals;
+  int ntpl, tpl_maxlen, use_tpl;
   const PlanEntry* dev;
   // row chunks for pipelined host<->device SpMV: chunk c = tiles [ctile[c], ctile[c+1]), rows [crow[c], crow[c+1]),
   // reading x only inside [ccol_lo[c], ccol_hi[c])
@@ -446,6 +595,9 @@ static int plan_create_impl(int vt, int it, int pt, int64_t nrows, int64_t ncols
   h->use_packed = 0;
   h->pk = PackedTiles{nullptr, nullptr, nullptr, nullptr, 0, 0};
   h->coded_vals = nullptr;
+  h->tpl = nullptr;
+  h->tpl_vals = nullptr;
+  h->ntpl = h->tpl_maxlen = h->use_tpl = 0;
   if (flavor == 2 && cfg_packable(cfg, vt) && kCfgs[cfg].kind == 1 && ntiles > 0 && nnz > 0) {
     B2S_CUDA(cudaMemsetAsync(stat, 0, 16, st));
     if (int rc = launch_pack<false>(it, pt, indptr, indices, dev, ntiles, h->pk, stat, nullptr, 0, DictBits{}, st)) {
@@ -640,16 +792,146 @@ int b2s_spmv_plan_pack_coded(void* plan, const void* indptr, const void* indices
   return pack_write(h, indptr, indices, coded ? vals : nullptr, vb, d, buf_dev, st);
 }
 
+/* Size of the device buffer b2s_spmv_plan_templates needs; 0 when the plan cannot run row templates: they stand in for
+ * the one-lane-per-row TMA kernel only, whose sums they reproduce bit for bit, so every tile must take that path. */
+int64_t b2s_spmv_plan_templates_bytes(const void* plan) {
+  const PlanHandle* h = (const PlanHandle*)plan;
+  if (!h || h->magic != kPlanMagic || h->flavor != 2 || kCfgs[h->cfg].kind != 1) return 0;
+  if (h->nrows <= 0 || h->nnz <= 0 || h->ntiles <= 0 || h->short_tiles != h->ntiles) return 0;
+  return kTplIdsOff + round16(h->nrows);
+}
+
+/* Row templates (TemplateTable): when every row has at most 8 entries and the rows have at most 32 distinct signatures,
+ * writes the table and one uint8 id per row into buf_dev (b2s_spmv_plan_templates_bytes bytes, 16-byte aligned,
+ * caller-owned, kept alive and unchanged as long as the plan is used) and switches whole-matrix launches with this
+ * `vals` pointer to the template kernel.  Otherwise the plan is left as it was.  Two host syncs. */
+int b2s_spmv_plan_templates(void* plan, const void* indptr, const void* indices, const void* vals, void* buf_dev,
+                            void* stream) {
+  PlanHandle* h = (PlanHandle*)plan;
+  B2S_CHECK_ARG(h && h->magic == kPlanMagic, "bad plan handle");
+  B2S_CHECK_ARG(b2s_spmv_plan_templates_bytes(h) > 0, "this plan cannot run row templates");
+  B2S_CHECK_ARG(indptr && indices && vals, "indptr / indices / vals is NULL");
+  B2S_CHECK_ARG(buf_dev != nullptr && aligned16(buf_dev), "template buffer must be non-NULL and 16-byte aligned");
+  B2S_CHECK_ARG(h->tpl == nullptr, "the plan already has row templates");
+  constexpr int CAP = kMaxTemplates + 1;
+  cudaStream_t st = (cudaStream_t)stream;
+  const int vbytes = h->vt == B2S_F32 ? 4 : 8;
+  const int64_t nrows = h->nrows;
+  const int64_t blocks64 = (nrows + 255) / 256;
+  const int blocks = (int)(blocks64 < kTplBlocks ? blocks64 : kTplBlocks);
+  // scratch: per-block hashes + representative rows + counts, then the merged representatives and the bad flag
+  const size_t tab_b = sizeof(unsigned long long) * CAP * (size_t)blocks;
+  const size_t cnt_off = 2 * tab_b, reps_off = round16(cnt_off + sizeof(int) * (size_t)blocks);
+  const size_t bad_off = reps_off + sizeof(long long) * kMaxTemplates;
+  unsigned char* tmp = nullptr;
+  B2S_CUDA(cudaMallocAsync((void**)&tmp, bad_off + 16, st));
+  unsigned long long* tabs = (unsigned long long*)tmp;
+  long long* breps = (long long*)(tmp + tab_b);
+  int* counts = (int*)(tmp + cnt_off);
+  long long* reps = (long long*)(tmp + reps_off);
+  int* bad = (int*)(tmp + bad_off);
+  const int it = h->it, pt = h->pt;
+#define B2S_TPL_LAUNCH(KERNEL, GRID, BLOCK, ...)                                                                      \
+  do {                                                                                                               \
+    if (it == B2S_I32 && pt == B2S_I32)                                                                              \
+      KERNEL<int32_t, int32_t><<<GRID, BLOCK, 0, st>>>(nrows, (const int32_t*)indptr, (const int32_t*)indices, __VA_ARGS__); \
+    else if (it == B2S_I32)                                                                                          \
+      KERNEL<int32_t, int64_t><<<GRID, BLOCK, 0, st>>>(nrows, (const int64_t*)indptr, (const int32_t*)indices, __VA_ARGS__); \
+    else if (pt == B2S_I32)                                                                                          \
+      KERNEL<int64_t, int32_t><<<GRID, BLOCK, 0, st>>>(nrows, (const int32_t*)indptr, (const int64_t*)indices, __VA_ARGS__); \
+    else                                                                                                             \
+      KERNEL<int64_t, int64_t><<<GRID, BLOCK, 0, st>>>(nrows, (const int64_t*)indptr, (const int64_t*)indices, __VA_ARGS__); \
+  } while (0)
+  // pass 1: per-block signature hashes, merged on the host
+  B2S_TPL_LAUNCH(tpl_collect_kernel, blocks, 256, vals, vbytes, tabs, breps, counts);
+  cudaError_t le = cudaGetLastError();
+  std::vector<unsigned long long> host_tabs((size_t)CAP * blocks);
+  std::vector<long long> host_reps((size_t)CAP * blocks);
+  std::vector<int> host_counts(blocks);
+  if (le == cudaSuccess) le = cudaMemcpyAsync(host_tabs.data(), tabs, tab_b, cudaMemcpyDeviceToHost, st);
+  if (le == cudaSuccess) le = cudaMemcpyAsync(host_reps.data(), breps, tab_b, cudaMemcpyDeviceToHost, st);
+  if (le == cudaSuccess) le = cudaMemcpyAsync(host_counts.data(), counts, sizeof(int) * blocks, cudaMemcpyDeviceToHost, st);
+  if (le == cudaSuccess) le = cudaStreamSynchronize(st);
+  if (le != cudaSuccess) { cudaFreeAsync(tmp, st); B2S_CUDA(le); }
+  std::vector<std::pair<unsigned long long, long long>> all;   // (hash, smallest representative row)
+  bool fits = true;
+  for (int b = 0; b < blocks && fits; b++) {
+    if (host_counts[b] > kMaxTemplates) fits = false;
+    for (int i = 0; fits && i < host_counts[b]; i++)
+      all.emplace_back(host_tabs[(size_t)CAP * b + i], host_reps[(size_t)CAP * b + i]);
+  }
+  std::sort(all.begin(), all.end());
+  all.erase(std::unique(all.begin(), all.end(), [](const auto& a, const auto& b) { return a.first == b.first; }),
+            all.end());
+  const int n = (int)all.size();
+  if (!fits || n == 0 || n > kMaxTemplates) { B2S_CUDA(cudaFreeAsync(tmp, st)); return B2S_OK; }
+  // the table from the representative rows, then pass 2: every row compared with its template
+  long long reps_host[kMaxTemplates];
+  for (int i = 0; i < n; i++) reps_host[i] = all[i].second;
+  TemplateTable* tab = (TemplateTable*)buf_dev;
+  uint8_t* ids = (uint8_t*)buf_dev + kTplIdsOff;
+  int lens[kMaxTemplates + 1] = {0};   // lengths, then the bad flag
+  le = cudaMemsetAsync(buf_dev, 0, sizeof(TemplateTable), st);
+  if (le == cudaSuccess) le = cudaMemsetAsync(bad, 0, sizeof(int), st);
+  if (le == cudaSuccess) le = cudaMemcpyAsync(reps, reps_host, sizeof(long long) * n, cudaMemcpyHostToDevice, st);
+  if (le == cudaSuccess) {
+    if (it == B2S_I32 && pt == B2S_I32)
+      tpl_table_kernel<int32_t, int32_t><<<1, 32, 0, st>>>((const int32_t*)indptr, (const int32_t*)indices, vals, vbytes, reps, n, tab);
+    else if (it == B2S_I32)
+      tpl_table_kernel<int32_t, int64_t><<<1, 32, 0, st>>>((const int64_t*)indptr, (const int32_t*)indices, vals, vbytes, reps, n, tab);
+    else if (pt == B2S_I32)
+      tpl_table_kernel<int64_t, int32_t><<<1, 32, 0, st>>>((const int32_t*)indptr, (const int64_t*)indices, vals, vbytes, reps, n, tab);
+    else
+      tpl_table_kernel<int64_t, int64_t><<<1, 32, 0, st>>>((const int64_t*)indptr, (const int64_t*)indices, vals, vbytes, reps, n, tab);
+    B2S_TPL_LAUNCH(tpl_assign_kernel, (unsigned)((nrows + 255) / 256), 256, vals, vbytes, tab, n, ids, bad);
+    le = cudaGetLastError();
+  }
+#undef B2S_TPL_LAUNCH
+  const int* dev_lens = (const int*)((const unsigned char*)buf_dev + offsetof(TemplateTable, len));
+  if (le == cudaSuccess) le = cudaMemcpyAsync(lens, dev_lens, sizeof(int) * kMaxTemplates, cudaMemcpyDeviceToHost, st);
+  if (le == cudaSuccess) le = cudaMemcpyAsync(lens + kMaxTemplates, bad, sizeof(int), cudaMemcpyDeviceToHost, st);
+  if (le == cudaSuccess) le = cudaStreamSynchronize(st);
+  cudaFreeAsync(tmp, st);
+  B2S_CUDA(le);
+  if (lens[kMaxTemplates]) return B2S_OK;
+  int maxlen = 0;
+  for (int i = 0; i < n; i++) maxlen = lens[i] > maxlen ? lens[i] : maxlen;
+  h->tpl = tab;
+  h->tpl_vals = vals;
+  h->ntpl = n;
+  h->tpl_maxlen = maxlen;
+  h->use_tpl = 1;
+  return B2S_OK;
+}
+
 /* tools / tests: 0 = launches stream the CSR arrays, 1 = the packed structure and the values, 2 = the packed structure
- * with coded values (the plan must have been packed / coded) */
+ * with coded values (the plan must have been packed / coded), 3 = row templates for whole-matrix launches (the plan must
+ * have them), with the other launches on the coded, else packed, else CSR kernel */
 int b2s_spmv_plan_set_packed(void* plan, int mode) {
   PlanHandle* h = (PlanHandle*)plan;
   B2S_CHECK_ARG(h && h->magic == kPlanMagic, "bad plan handle");
-  B2S_CHECK_ARG(mode >= 0 && mode <= 2, "mode must be 0, 1 or 2");
-  B2S_CHECK_ARG(!mode || h->pk.cols != nullptr, "the plan has not been packed (b2s_spmv_plan_pack)");
+  B2S_CHECK_ARG(mode >= 0 && mode <= 3, "mode must be 0, 1, 2 or 3");
+  B2S_CHECK_ARG(!mode || mode == 3 || h->pk.cols != nullptr, "the plan has not been packed (b2s_spmv_plan_pack)");
   B2S_CHECK_ARG(mode != 2 || h->pk.dict != nullptr, "the plan's values are not coded (b2s_spmv_plan_pack_coded)");
-  h->use_packed = mode;
+  B2S_CHECK_ARG(mode != 3 || h->tpl != nullptr, "the plan has no row templates (b2s_spmv_plan_templates)");
+  h->use_tpl = mode == 3 ? 1 : 0;
+  h->use_packed = mode == 3 ? (h->pk.dict ? 2 : (h->pk.cols ? 1 : 0)) : mode;
   return B2S_OK;
+}
+
+/* tuning hook (tools): shape of the row-template kernel -- rows per lane (1, 2), threads per CTA (128, 256) and
+ * evict-first y stores (1); 0 restores the default */
+int b2s_spmv_set_template_config(int rows, int threads, int streaming) {
+  B2S_CHECK_ARG(rows == 0 || rows == 1 || rows == 2, "rows per lane must be 1 or 2");
+  B2S_CHECK_ARG(threads == 0 || threads == 128 || threads == 256, "threads must be 128 or 256");
+  g_tpl_rows.store(rows);
+  g_tpl_threads.store(threads);
+  g_tpl_streaming.store(streaming ? 1 : 0);
+  return B2S_OK;
+}
+
+static bool plan_runs_templates(const PlanHandle* h) {
+  return h->use_tpl && h->tpl != nullptr && !h->use_rowgroup && h->flavor == 2 && kCfgs[h->cfg].kind == 1;
 }
 
 static bool plan_runs_packed(const PlanHandle* h) {
@@ -657,14 +939,16 @@ static bool plan_runs_packed(const PlanHandle* h) {
 }
 
 /* out[0] = tile config, out[1] = bit0 row-group kernel forced, bit1 uniform-row flavour, bit2 scattered, bit3 short-row
- * flavour, bit4 TMA kind, bit5 packed structure, bit6 coded values, bits 8..12 distinct values of a coded plan;
- * out[2] = ntiles, out[3] = 1000 * mean distinct x lines per 32 consecutive nonzeros */
+ * flavour, bit4 TMA kind, bit5 packed structure, bit6 coded values, bit7 row templates, bits 8..12 distinct values of a
+ * coded plan, bits 16..23 row templates of the plan; out[2] = ntiles, out[3] = 1000 * mean distinct x lines per 32
+ * consecutive nonzeros */
 int b2s_spmv_plan_info(const void* plan, int64_t* out4_host) {
   const PlanHandle* h = (const PlanHandle*)plan;
   B2S_CHECK_ARG(h && h->magic == kPlanMagic && out4_host, "bad plan handle / out pointer");
   out4_host[0] = h->cfg;
   out4_host[1] = h->use_rowgroup + 2 * (h->flavor == 1) + 4 * h->scattered + 8 * (h->flavor == 2) + 16 * (kCfgs[h->cfg].kind == 1) +
-                 32 * plan_runs_packed(h) + 64 * (plan_runs_packed(h) && h->use_packed == 2) + 256 * (int64_t)h->pk.ndict;
+                 32 * plan_runs_packed(h) + 64 * (plan_runs_packed(h) && h->use_packed == 2) +
+                 128 * plan_runs_templates(h) + 256 * (int64_t)h->pk.ndict + 65536 * (int64_t)h->ntpl;
   out4_host[2] = h->ntiles;
   out4_host[3] = (int64_t)(h->lines_per_warp * 1000.0);
   return B2S_OK;
@@ -720,6 +1004,23 @@ static int spmv_impl(int vt, int it, int pt, int64_t nrows, int64_t ncols, int64
                              : spmv_rowgroup_f64(it, pt, nrows, nnz, indptr, indices, vals, x, y, st);
     if (rc || !dot) return rc;
     return b2s_dot(vt, nrows, w, y, dot_out, ws, stream);
+  }
+  // row templates: whole-matrix products (b2s_spmv_csr / _dot: no tile range, exchange or accumulation) with the values
+  // the templates were built from; every other launch of the plan keeps the tile kernels, which compute the same y
+  if (plan_runs_templates(h) && tile_hi < 0 && !order && !accumulate && vals == h->tpl_vals) {
+    TemplateLaunch t;
+    t.tab = h->tpl;
+    t.ids = (const uint8_t*)h->tpl + kTplIdsOff;
+    t.nrows = nrows;
+    t.maxlen = h->tpl_maxlen;
+    const int rows = g_tpl_rows.load(), threads = g_tpl_threads.load();
+    t.rows = rows > 0 ? rows : kTplRowsDefault;
+    t.threads = threads > 0 ? threads : kTplThreadsDefault;
+    t.streaming = g_tpl_streaming.load();
+    t.x = x; t.y = y;
+    t.w = dot ? w : nullptr; t.dot_out = dot ? dot_out : nullptr; t.ws = dot ? ws : nullptr;
+    t.st = st;
+    return vt == B2S_F32 ? spmv_template_f32(dot, t) : spmv_template_f64(dot, t);
   }
   SpmvArgs a;
   a.ntiles = h->ntiles;

@@ -131,6 +131,23 @@ struct PackedTiles {
 };
 constexpr int kPackColGap = 16, kPackRowGap = 8;
 
+// Row templates (b2s_spmv_plan_templates).  The signature of row r is its length, then indices[k] - r for its entries
+// in stored order, then the bit patterns of their values.  When every row has at most kTplLen entries and the matrix has
+// at most kMaxTemplates distinct signatures (the 9 of a 5-point Laplacian, the 27 of a 3-D 7-point stencil), a plan
+// keeps the signatures in a table and one uint8 template id per row, and a whole-matrix product streams only the ids,
+// x and y.  Templates are sorted by signature hash, so the ids of a matrix do not depend on the run.
+constexpr int kMaxTemplates = 32, kTplLen = 8;
+struct __align__(16) TemplateTable {
+  unsigned long long bits[kMaxTemplates][kTplLen];   // value bit patterns (fp32: the low 32 bits); 0 past the length
+  unsigned long long hash[kMaxTemplates];            // signature hashes (ascending; plan time only)
+  int off[kMaxTemplates][kTplLen];                   // column - row; 0 past the length
+  int len[kMaxTemplates];
+};
+// the template buffer: the table, then ids[nrows]
+constexpr int64_t kTplIdsOff = (sizeof(TemplateTable) + 15) & ~(size_t)15;
+// default kernel shape: rows per lane, threads per CTA (DESIGN.md 8)
+constexpr int kTplRowsDefault = 1, kTplThreadsDefault = 256;
+
 struct SpmvArgs {
   int64_t ntiles, nrows, nnz;
   PackedTiles pk;            // all NULL = the matrix is not packed (or packing is switched off)
@@ -156,5 +173,22 @@ int spmv_rowgroup_f32(int it, int pt, int64_t nrows, int64_t nnz, const void* in
                       const void* vals, const void* x, void* y, cudaStream_t st);
 int spmv_rowgroup_f64(int it, int pt, int64_t nrows, int64_t nnz, const void* indptr, const void* indices,
                       const void* vals, const void* x, void* y, cudaStream_t st);
+
+// Row-template product (see TemplateTable): maxlen = longest template, rows = rows per lane (1, 2), threads per
+// CTA, streaming = evict-first y stores.  Without dot, w / dot_out / ws are unused.
+struct TemplateLaunch {
+  const TemplateTable* tab;
+  const uint8_t* ids;
+  int64_t nrows;
+  int maxlen, rows, threads, streaming;
+  const void* x;
+  void* y;
+  const void* w;
+  void* dot_out;
+  void* ws;
+  cudaStream_t st;
+};
+int spmv_template_f32(bool dot, const TemplateLaunch& a);
+int spmv_template_f64(bool dot, const TemplateLaunch& a);
 
 }  // namespace b2s

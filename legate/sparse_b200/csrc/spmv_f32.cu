@@ -14,4 +14,8 @@ int spmv_rowgroup_f32(int it, int pt, int64_t nrows, int64_t nnz, const void* in
   return dispatch_rowgroup<float>(it, pt, nrows, nnz, indptr, indices, vals, x, y, st);
 }
 
+int spmv_template_f32(bool dot, const TemplateLaunch& a) {
+  return dot ? launch_template<float, true>(a) : launch_template<float, false>(a);
+}
+
 }  // namespace b2s

@@ -14,4 +14,8 @@ int spmv_rowgroup_f64(int it, int pt, int64_t nrows, int64_t nnz, const void* in
   return dispatch_rowgroup<double>(it, pt, nrows, nnz, indptr, indices, vals, x, y, st);
 }
 
+int spmv_template_f64(bool dot, const TemplateLaunch& a) {
+  return dot ? launch_template<double, true>(a) : launch_template<double, false>(a);
+}
+
 }  // namespace b2s

@@ -910,6 +910,78 @@ spmv_rowgroup_kernel(int64_t nrows, const P* __restrict__ indptr, const I* __res
 }
 
 // ---------------------------------------------------------------------------------------------
+// Row templates (TemplateTable): y[r] = sum_j val[t][j] * x[r + off[t][j]] with t = ids[r].  No matrix stream but one
+// byte per row, so no staging ring either: the table sits in shared memory, a warp takes chunks of 32 R consecutive
+// rows (lane l: rows l + 32 q) and issues the gathers of all its R rows before the first FMA.  A grid of resident CTAs
+// walks the chunks in row order, so the rows in flight span a few MB of x and its +-n1 neighbours stay in L2.
+// Each sum is formed exactly as the one-lane-per-row CSR path forms it (short_row_sum: U terms from +0 in stored order,
+// zero products past the row's end, then + 0.0 in place of the old y), so y is bit-identical to the other kernels of
+// the same plan -- up to which NaN survives where two different NaNs meet in one FMA (an inf - inf sum times a NaN in
+// x), which follows the operand order the compiler picked for that FMA.
+// ---------------------------------------------------------------------------------------------
+// 64 warps per SM: at most 32 registers.
+template <typename V, int U, int R, int THREADS, bool DOT>
+__global__ void __launch_bounds__(THREADS, 2048 / THREADS)
+spmv_template_kernel(int64_t nrows, const uint8_t* __restrict__ ids, const TemplateTable* __restrict__ tab,
+                     const V* __restrict__ x, V* __restrict__ y, int streaming, const V* __restrict__ w, V* dot_out,
+                     void* ws) {
+  __shared__ int soff[kMaxTemplates][U];
+  __shared__ V sval[kMaxTemplates][U];
+  __shared__ int slen[kMaxTemplates];
+  __shared__ double red[32];
+  __shared__ bool s_flag;
+  for (int i = threadIdx.x; i < kMaxTemplates * U; i += THREADS) {
+    const int t = i / U, j = i % U;
+    soff[t][j] = tab->off[t][j];
+    const unsigned long long b = tab->bits[t][j];
+    if constexpr (sizeof(V) == 8) sval[t][j] = __longlong_as_double((long long)b);
+    else                          sval[t][j] = __uint_as_float((unsigned)b);
+  }
+  if (threadIdx.x < kMaxTemplates) slen[threadIdx.x] = tab->len[threadIdx.x];
+  __syncthreads();
+  constexpr int WPB = THREADS / 32;
+  const int lane = threadIdx.x & 31;
+  const int64_t nchunks = (nrows + 32 * R - 1) / (32 * R);
+  double dot_acc = 0.0;
+  for (int64_t c = (int64_t)blockIdx.x * WPB + (threadIdx.x >> 5); c < nchunks; c += (int64_t)gridDim.x * WPB) {
+    const int64_t r0 = c * (32 * R) + lane;
+    int t[R], n[R];
+#pragma unroll
+    for (int q = 0; q < R; q++) {
+      const int64_t r = r0 + 32 * q;
+      t[q] = r < nrows ? (int)__ldcs(ids + r) : 0;
+      n[q] = r < nrows ? slen[t[q]] : 0;
+    }
+    V xv[R][U];
+#pragma unroll
+    for (int q = 0; q < R; q++) {
+#pragma unroll
+      for (int j = 0; j < U; j++) xv[q][j] = j < n[q] ? __ldg(x + (r0 + 32 * q + soff[t[q]][j])) : (V)0;
+    }
+#pragma unroll
+    for (int q = 0; q < R; q++) {
+      V acc = (V)0;
+#pragma unroll
+      for (int j = 0; j < U; j++) acc += (j < n[q] ? sval[t[q]][j] : (V)0) * xv[q][j];
+      acc += (V)0;   // the CSR path's "+ old y" of a plain product: -0.0 -> +0.0 exactly as there
+      const int64_t r = r0 + 32 * q;
+      if (r < nrows) {
+        if (streaming) __stcs(y + r, acc);
+        else           y[r] = acc;
+        if (DOT) dot_acc += (double)acc * (double)w[r];
+      }
+    }
+  }
+  if (DOT) {
+    double part = block_sum<THREADS>(dot_acc, red);
+    if (grid_reduce_is_last<THREADS>(ws, part, red, &s_flag)) {
+      double total = grid_reduce_final<THREADS>(ws, red);
+      if (threadIdx.x == 0) *dot_out = (V)total;
+    }
+  }
+}
+
+// ---------------------------------------------------------------------------------------------
 // Host-side launchers.  Kernel attributes / occupancy are cached per (instantiation, device) under a mutex:
 // the library is re-entrant per (device, stream) and may be called from one host thread per GPU.
 // ---------------------------------------------------------------------------------------------
@@ -1087,6 +1159,45 @@ static int dispatch_rowgroup(int it, int pt, int64_t nrows, int64_t nnz, const v
   if (it == B2S_I64 && pt == B2S_I64) return launch_rowgroup<V, int64_t, int64_t>(nrows, nnz, indptr, indices, vals, x, y, st);
   set_error("bad index type codes it=%d pt=%d", it, pt);
   return B2S_EINVAL;
+}
+
+// Row-template launches: one resident wave of CTAs (occupancy x SMs) walking the row chunks in order.
+template <typename V, int U, int R, int THREADS, bool DOT>
+static int launch_template_f(const TemplateLaunch& a) {
+  auto kern = spmv_template_kernel<V, U, R, THREADS, DOT>;
+  static LaunchCache cache;
+  int occ = 1;
+  if (int rc = launch_prepare(cache, kern, THREADS, 0, &occ)) return rc;
+  DeviceProps pr;
+  if (int rc = get_props(&pr)) return rc;
+  const int64_t chunks_per_cta = (int64_t)(THREADS / 32);
+  const int64_t want = (a.nrows + 32 * R * chunks_per_cta - 1) / (32 * R * chunks_per_cta);
+  int64_t grid = (int64_t)pr.sm_count * occ;
+  if (DOT && grid > WS_MAX_PARTIALS) grid = WS_MAX_PARTIALS;
+  if (grid > want) grid = want;
+  if (grid < 1) grid = 1;
+  kern<<<(unsigned)grid, THREADS, 0, a.st>>>(a.nrows, a.ids, a.tab, (const V*)a.x, (V*)a.y, a.streaming,
+                                             (const V*)a.w, (V*)a.dot_out, a.ws);
+  B2S_LAUNCH_CHECK();
+  return B2S_OK;
+}
+
+// Instantiated: rows of up to 5 entries at R in {1, 2} and 128 / 256 threads (the sweep in DESIGN.md 8); longer rows
+// (up to kTplLen) at one row per lane and 256 threads whatever the tuning hook asks, so they keep 64 warps per SM.
+template <typename V, bool DOT>
+static int launch_template(const TemplateLaunch& a) {
+  if (a.maxlen > 5) {
+    return launch_template_f<V, kTplLen, 1, 256, DOT>(a);
+  } else if (a.threads == 256) {
+    if (a.rows == 1) return launch_template_f<V, 5, 1, 256, DOT>(a);
+    if (a.rows == 2) return launch_template_f<V, 5, 2, 256, DOT>(a);
+  } else if (a.threads == 128) {
+    if (a.rows == 1) return launch_template_f<V, 5, 1, 128, DOT>(a);
+    if (a.rows == 2) return launch_template_f<V, 5, 2, 128, DOT>(a);
+  }
+  set_error("no row-template kernel is built for %d rows per lane, %d threads and rows of %d entries", a.rows, a.threads,
+            a.maxlen);
+  return B2S_EUNSUPPORTED;
 }
 
 }  // namespace b2s

@@ -1,5 +1,5 @@
-"""Kernel-level A/B/C of the SpMV structure encodings -- coded values, packed structure, CSR arrays -- next to a streaming
-ceiling.
+"""Kernel-level A/B/C of the SpMV structure encodings -- row templates, coded values, packed structure, CSR arrays -- next
+to a streaming ceiling.
 
     python tools/bench_packed.py [--launches 200] [--reps 5] [--out DIR]
 
@@ -46,9 +46,12 @@ def csr_bytes(A):
 
 def moved_bytes(A, plan, mode):
     """Bytes one launch streams: per tile the plan entry, and either the staged 16-byte groups of indices / indptr or
-    the packed uint16 slices plus the tile base; values (none when coded: mode 2), x once and y once."""
+    the packed uint16 slices plus the tile base; values (none when coded: mode 2), x once and y once.  Row templates
+    (mode 3): one id byte per row, x once and y once."""
     sv, si, sp = A.data.element_size(), A.indices.element_size(), A.indptr.element_size()
     n, m = A.shape
+    if mode == 3:
+        return n + m * sv + n * sv
     e = plan.buf[: 4 * (plan.tiles + 1)].view(-1, 4).cpu().numpy().astype(np.int64)
     k = (e[:, 0] & 0xFFFFFFFF) | (e[:, 1] << 32)
     r = e[:, 2]
@@ -98,8 +101,9 @@ def main():
         def run(A=A, plan=plan, x=x, y=y):
             _ops.spmv(A.indptr, A.indices, A.data, x, y, A.shape, plan=plan)
 
-        for mode in ([2, 1, 0] if plan.coded else [1, 0] if plan.packed else [0]):
-            cases[f"{name}_{('csr', 'packed', 'coded')[mode]}"] = dict(
+        modes = [2, 1, 0] if plan.coded else [1, 0] if plan.packed else [0]
+        for mode in ([3] if plan.templated else []) + modes:
+            cases[f"{name}_{('csr', 'packed', 'coded', 'templates')[mode]}"] = dict(
                 run=run, plan=plan, mode=mode, csr=csr_bytes(A), moved=moved_bytes(A, plan, mode),
                 flops=2 * A.nnz, kernel=None)
     probe = torch.rand(200_000_000, dtype=torch.float64, device="cuda")   # 1.6 GB
@@ -148,6 +152,9 @@ def main():
         if f"{m}_coded" in rows:
             print(f"# {m}: packed / coded time = {rows[f'{m}_packed']['us_median'] / rows[f'{m}_coded']['us_median']:.3f}, "
                   f"csr / coded = {rows[f'{m}_csr']['us_median'] / rows[f'{m}_coded']['us_median']:.3f}")
+        if f"{m}_templates" in rows and f"{m}_coded" in rows:
+            print(f"# {m}: coded / templates time = "
+                  f"{rows[f'{m}_coded']['us_median'] / rows[f'{m}_templates']['us_median']:.3f}")
     if args.out:
         os.makedirs(args.out, exist_ok=True)
         with open(os.path.join(args.out, "bench_packed.json"), "w") as f:
