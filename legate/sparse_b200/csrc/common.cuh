@@ -31,6 +31,29 @@ void set_error(const char* fmt, ...);
 
 #define B2S_LAUNCH_CHECK() B2S_CUDA(cudaGetLastError())
 
+// ---- ABI type codes to C++ types ----------------------------------------------------
+// Each calls `f` with a value of the type a code names (`using V = decltype(v);` recovers it) and returns f's int.  An
+// unknown code sets an error and returns B2S_EINVAL; entry points check their codes first, with their own messages.
+template <typename F>
+inline int with_value_type(int vt, F&& f) {
+  if (vt == B2S_F32) return f(float{});
+  if (vt == B2S_F64) return f(double{});
+  set_error("bad value type code %d", vt);
+  return B2S_EINVAL;
+}
+template <typename F>
+inline int with_index_type(int it, F&& f) {
+  if (it == B2S_I32) return f(int32_t{});
+  if (it == B2S_I64) return f(int64_t{});
+  set_error("bad index type code %d", it);
+  return B2S_EINVAL;
+}
+// column index type `it`, row pointer type `pt`: f(I{}, P{})
+template <typename F>
+inline int with_index_types(int it, int pt, F&& f) {
+  return with_index_type(it, [&](auto i) { return with_index_type(pt, [&](auto p) { return f(i, p); }); });
+}
+
 struct DeviceProps {
   int sm_count;
   int max_smem_optin;

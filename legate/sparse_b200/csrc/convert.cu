@@ -275,17 +275,13 @@ int b2s_coo_to_csr(int vt, int it, int pt, int64_t nrows, int64_t nnz, const voi
   B2S_CHECK_ARG(pt == B2S_I64 || nnz < 2147483647LL, "int32 indptr cannot address nnz >= 2^31-1");
   cudaStream_t st = (cudaStream_t)stream;
   unsigned char* sc = (unsigned char*)scratch;
-#define B2S_CV(V, I, P) return cv_run<V, I, P, P, false>(nrows, nnz, (const I*)rows, (const I*)cols, (const V*)vals, (const P*)nullptr, 0, \
-                                                         (P*)indptr, (I*)indices, (V*)vals_out, sc, bad_host, st)
-  if (vt == B2S_F32) {
-    if (it == B2S_I32) { if (pt == B2S_I32) B2S_CV(float, int32_t, int32_t); B2S_CV(float, int32_t, int64_t); }
-    if (pt == B2S_I32) B2S_CV(float, int64_t, int32_t);
-    B2S_CV(float, int64_t, int64_t);
-  }
-  if (it == B2S_I32) { if (pt == B2S_I32) B2S_CV(double, int32_t, int32_t); B2S_CV(double, int32_t, int64_t); }
-  if (pt == B2S_I32) B2S_CV(double, int64_t, int32_t);
-  B2S_CV(double, int64_t, int64_t);
-#undef B2S_CV
+  return with_value_type(vt, [&](auto v) {
+    return with_index_types(it, pt, [&](auto i, auto p) {
+      using V = decltype(v); using I = decltype(i); using P = decltype(p);
+      return cv_run<V, I, P, P, false>(nrows, nnz, (const I*)rows, (const I*)cols, (const V*)vals, (const P*)nullptr, 0,
+                                       (P*)indptr, (I*)indices, (V*)vals_out, sc, bad_host, st);
+    });
+  });
 }
 
 /* CSR (nrows x ncols) -> CSR of the transpose (ncols x nrows), rows sorted.  Input and output share the index width
@@ -301,20 +297,14 @@ int b2s_csr_transpose(int vt, int it, int pt, int64_t nrows, int64_t ncols, int6
   cudaStream_t st = (cudaStream_t)stream;
   unsigned char* sc = (unsigned char*)scratch;
   int64_t bad = 0;
-#define B2S_CT(V, I, P) { int rc = cv_run<V, I, P, P, true>(ncols, nnz, (const I*)nullptr, (const I*)indices, (const V*)vals, (const P*)indptr, \
-                                                            nrows, (P*)t_indptr, (I*)t_indices, (V*)t_vals, sc, &bad, st);                  \
-                          if (rc) return rc; break; }
-  switch ((vt == B2S_F64 ? 4 : 0) + (it == B2S_I64 ? 2 : 0) + (pt == B2S_I64 ? 1 : 0)) {
-    case 0: B2S_CT(float, int32_t, int32_t)
-    case 1: B2S_CT(float, int32_t, int64_t)
-    case 2: B2S_CT(float, int64_t, int32_t)
-    case 3: B2S_CT(float, int64_t, int64_t)
-    case 4: B2S_CT(double, int32_t, int32_t)
-    case 5: B2S_CT(double, int32_t, int64_t)
-    case 6: B2S_CT(double, int64_t, int32_t)
-    default: B2S_CT(double, int64_t, int64_t)
-  }
-#undef B2S_CT
+  if (int rc = with_value_type(vt, [&](auto v) {
+        return with_index_types(it, pt, [&](auto i, auto p) {
+          using V = decltype(v); using I = decltype(i); using P = decltype(p);
+          return cv_run<V, I, P, P, true>(ncols, nnz, (const I*)nullptr, (const I*)indices, (const V*)vals,
+                                          (const P*)indptr, nrows, (P*)t_indptr, (I*)t_indices, (V*)t_vals, sc, &bad, st);
+        });
+      }))
+    return rc;
   B2S_CHECK_ARG(bad == 0, "%lld column indices outside [0, ncols)", (long long)bad);
   return B2S_OK;
 }
@@ -336,18 +326,12 @@ int b2s_csr_sort_rows(int vt, int it, int pt, int64_t nrows, int64_t nnz, const 
   unsigned long long* counters = (unsigned long long*)(sc + L.off_counters);
   int64_t* list = (int64_t*)(sc + L.off_list);
   B2S_CUDA(cudaMemsetAsync(counters, 0, 256, st));
-#define B2S_SR(V, I, P) return cv_sort_rows<V, I, P>(pr, nrows, nnz, (const P*)indptr, (I*)indices, (V*)vals, counters, list, nullptr, st)
-  switch ((vt == B2S_F64 ? 4 : 0) + (it == B2S_I64 ? 2 : 0) + (pt == B2S_I64 ? 1 : 0)) {
-    case 0: B2S_SR(float, int32_t, int32_t);
-    case 1: B2S_SR(float, int32_t, int64_t);
-    case 2: B2S_SR(float, int64_t, int32_t);
-    case 3: B2S_SR(float, int64_t, int64_t);
-    case 4: B2S_SR(double, int32_t, int32_t);
-    case 5: B2S_SR(double, int32_t, int64_t);
-    case 6: B2S_SR(double, int64_t, int32_t);
-    default: B2S_SR(double, int64_t, int64_t);
-  }
-#undef B2S_SR
+  return with_value_type(vt, [&](auto v) {
+    return with_index_types(it, pt, [&](auto i, auto p) {
+      using V = decltype(v); using I = decltype(i); using P = decltype(p);
+      return cv_sort_rows<V, I, P>(pr, nrows, nnz, (const P*)indptr, (I*)indices, (V*)vals, counters, list, nullptr, st);
+    });
+  });
 }
 
 }  // extern "C"

@@ -358,13 +358,13 @@ int b2s_csr_binop_symbolic(int op, int it, int pt, int64_t m, int64_t n, const v
   B2S_CUDA(cudaMemsetAsync(ctr, 0, 256, st));
   B2S_CUDA(cudaMemsetAsync(cp, 0, sizeof(long long), st));
   if (m > 0) {
-    int rc;
-#define B2S_EWS(I, P) rc = ew_run<false, float, I, P>(pr, op, m, a_indptr, a_indices, nullptr, b_indptr, b_indices, nullptr, cp, nullptr, nullptr, sc, st)
-    if (it == B2S_I32) { if (pt == B2S_I32) B2S_EWS(int32_t, int32_t); else B2S_EWS(int32_t, int64_t); }
-    else               { if (pt == B2S_I32) B2S_EWS(int64_t, int32_t); else B2S_EWS(int64_t, int64_t); }
-#undef B2S_EWS
-    if (rc) return rc;
-    if (int rc2 = cv_inclusive_scan<long long>(cp, m + 1, (long long*)(sc + L.off_sums), st)) return rc2;
+    // the symbolic pass reads no values: one instantiation (float) serves both value types
+    if (int rc = with_index_types(it, pt, [&](auto i, auto p) {
+          return ew_run<false, float, decltype(i), decltype(p)>(pr, op, m, a_indptr, a_indices, nullptr, b_indptr,
+                                                                b_indices, nullptr, cp, nullptr, nullptr, sc, st);
+        }))
+      return rc;
+    if (int rc = cv_inclusive_scan<long long>(cp, m + 1, (long long*)(sc + L.off_sums), st)) return rc;
   }
   long long nnz = 0;
   unsigned long long bad[2] = {0, 0};
@@ -392,18 +392,12 @@ int b2s_csr_binop_numeric(int op, int vt, int it, int pt, int64_t m, int64_t n, 
   cudaStream_t st = (cudaStream_t)stream;
   unsigned char* sc = (unsigned char*)scratch;
   long long* cp = (long long*)const_cast<int64_t*>(c_indptr);
-#define B2S_EWN(V, I, P) return ew_run<true, V, I, P>(pr, op, m, a_indptr, a_indices, a_vals, b_indptr, b_indices, b_vals, cp, c_indices, c_vals, sc, st)
-  switch ((vt == B2S_F64 ? 4 : 0) + (it == B2S_I64 ? 2 : 0) + (pt == B2S_I64 ? 1 : 0)) {
-    case 0: B2S_EWN(float, int32_t, int32_t);
-    case 1: B2S_EWN(float, int32_t, int64_t);
-    case 2: B2S_EWN(float, int64_t, int32_t);
-    case 3: B2S_EWN(float, int64_t, int64_t);
-    case 4: B2S_EWN(double, int32_t, int32_t);
-    case 5: B2S_EWN(double, int32_t, int64_t);
-    case 6: B2S_EWN(double, int64_t, int32_t);
-    default: B2S_EWN(double, int64_t, int64_t);
-  }
-#undef B2S_EWN
+  return with_value_type(vt, [&](auto v) {
+    return with_index_types(it, pt, [&](auto i, auto p) {
+      return ew_run<true, decltype(v), decltype(i), decltype(p)>(pr, op, m, a_indptr, a_indices, a_vals, b_indptr,
+                                                                 b_indices, b_vals, cp, c_indices, c_vals, sc, st);
+    });
+  });
 }
 
 int b2s_csr_scale(int vt, int it, int pt, int64_t m, int64_t n, int64_t nnz, int mode, const void* indptr,
@@ -417,21 +411,15 @@ int b2s_csr_scale(int vt, int it, int pt, int64_t m, int64_t n, int64_t nnz, int
   if (m == 0 || nnz == 0) return B2S_OK;
   cudaStream_t st = (cudaStream_t)stream;
   const unsigned grid = (unsigned)((m + 255) / 256);
-#define B2S_SC(V, I, P) { ew_scale_kernel<V, I, P><<<grid, 256, 0, st>>>(m, (const P*)indptr, (const I*)indices, (const V*)vals, \
-                                                                  (const V*)d, ldd, mode, (V*)out_vals); break; }
-  switch ((vt == B2S_F64 ? 4 : 0) + (it == B2S_I64 ? 2 : 0) + (pt == B2S_I64 ? 1 : 0)) {
-    case 0: B2S_SC(float, int32_t, int32_t)
-    case 1: B2S_SC(float, int32_t, int64_t)
-    case 2: B2S_SC(float, int64_t, int32_t)
-    case 3: B2S_SC(float, int64_t, int64_t)
-    case 4: B2S_SC(double, int32_t, int32_t)
-    case 5: B2S_SC(double, int32_t, int64_t)
-    case 6: B2S_SC(double, int64_t, int32_t)
-    default: B2S_SC(double, int64_t, int64_t)
-  }
-#undef B2S_SC
-  B2S_LAUNCH_CHECK();
-  return B2S_OK;
+  return with_value_type(vt, [&](auto v) {
+    return with_index_types(it, pt, [&](auto i, auto p) {
+      using V = decltype(v); using I = decltype(i); using P = decltype(p);
+      ew_scale_kernel<V, I, P><<<grid, 256, 0, st>>>(m, (const P*)indptr, (const I*)indices, (const V*)vals, (const V*)d,
+                                                    ldd, mode, (V*)out_vals);
+      B2S_LAUNCH_CHECK();
+      return B2S_OK;
+    });
+  });
 }
 
 }  // extern "C"

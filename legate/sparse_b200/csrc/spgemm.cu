@@ -847,10 +847,12 @@ int b2s_spgemm_row_work(int pt, int64_t m, const void* a_indptr, const int32_t* 
   cudaStream_t st = (cudaStream_t)stream;
   int64_t want = (m * 32 + 255) / 256, cap = (int64_t)pr.sm_count * 32;
   unsigned grid = (unsigned)(want < cap ? want : cap);
-  if (pt == B2S_I32) spgemm_ub_kernel<int32_t><<<grid, 256, 0, st>>>(m, (const int32_t*)a_indptr, a_indices, (const int32_t*)b_indptr, (long long*)work_out);
-  else               spgemm_ub_kernel<int64_t><<<grid, 256, 0, st>>>(m, (const int64_t*)a_indptr, a_indices, (const int64_t*)b_indptr, (long long*)work_out);
-  B2S_LAUNCH_CHECK();
-  return B2S_OK;
+  return with_index_type(pt, [&](auto p) {
+    using P = decltype(p);
+    spgemm_ub_kernel<P><<<grid, 256, 0, st>>>(m, (const P*)a_indptr, a_indices, (const P*)b_indptr, (long long*)work_out);
+    B2S_LAUNCH_CHECK();
+    return B2S_OK;
+  });
 }
 
 int b2s_spgemm_csr_symbolic(int pt, int64_t m, int64_t k, int64_t n, const void* a_indptr, const int32_t* a_indices,
@@ -873,23 +875,20 @@ int b2s_spgemm_csr_symbolic(int pt, int64_t m, int64_t k, int64_t n, const void*
   info_host[0] = info_host[1] = info_host[2] = 0;
   B2S_CUDA(cudaMemsetAsync(c_indptr, 0, sizeof(int64_t) * (size_t)(m + 1), st));
   if (m == 0) { B2S_CUDA(cudaStreamSynchronize(st)); return B2S_OK; }
-  {
-    int64_t want = (m * 32 + 255) / 256, cap = (int64_t)pr.sm_count * 32;
-    unsigned grid = (unsigned)(want < cap ? want : cap);
-    if (pt == B2S_I32) spgemm_ub_kernel<int32_t><<<grid, 256, 0, st>>>(m, (const int32_t*)a_indptr, a_indices, (const int32_t*)b_indptr, ub);
-    else               spgemm_ub_kernel<int64_t><<<grid, 256, 0, st>>>(m, (const int64_t*)a_indptr, a_indices, (const int64_t*)b_indptr, ub);
-    B2S_LAUNCH_CHECK();
-  }
+  if (int rc = b2s_spgemm_row_work(pt, m, a_indptr, a_indices, b_indptr, (int64_t*)ub, stream)) return rc;
   unsigned long long counts[16] = {0};
   unsigned long long flops = 0;
   ClsOffsets offs;
   if (int rc = run_binning<false>(m, ub, hdr, perm, true, counts, &flops, &offs, st)) return rc;
   if (dense_total(counts)) B2S_CUDA(cudaMemsetAsync(bitmaps, 0, (size_t)(L.bitmap_slot_bytes * L.nslots), st));
-  int rc;
   long long* cp = (long long*)c_indptr;
-  if (pt == B2S_I32) rc = run_classes<float, int32_t, false>(pr.sm_count, counts, offs, perm, a_indptr, a_indices, nullptr, b_indptr, b_indices, nullptr, cp, nullptr, nullptr, bitmaps, L, nullptr, 0, n, hdr, st);
-  else               rc = run_classes<float, int64_t, false>(pr.sm_count, counts, offs, perm, a_indptr, a_indices, nullptr, b_indptr, b_indices, nullptr, cp, nullptr, nullptr, bitmaps, L, nullptr, 0, n, hdr, st);
-  if (rc) return rc;
+  // the symbolic pass reads no values: one instantiation (float) serves both value types
+  if (int rc = with_index_type(pt, [&](auto p) {
+        return run_classes<float, decltype(p), false>(pr.sm_count, counts, offs, perm, a_indptr, a_indices, nullptr,
+                                                      b_indptr, b_indices, nullptr, cp, nullptr, nullptr, bitmaps, L,
+                                                      nullptr, 0, n, hdr, st);
+      }))
+    return rc;
   if (int rc2 = run_scan(cp, m + 1, bsums, st)) return rc2;
   long long nnz = 0;
   B2S_CUDA(cudaMemcpyAsync(&nnz, cp + m, sizeof(long long), cudaMemcpyDeviceToHost, st));
@@ -933,12 +932,13 @@ int b2s_spgemm_csr_numeric(int vt, int pt, int64_t m, int64_t k, int64_t n, cons
     B2S_CUDA(cudaMemsetAsync(dense_ws, 0, (size_t)(dense_slots * per), st));
   }
   long long* cp = (long long*)const_cast<int64_t*>(c_indptr);
-  if (vt == B2S_F32) {
-    if (pt == B2S_I32) return run_classes<float, int32_t, true>(pr.sm_count, counts, offs, perm, a_indptr, a_indices, a_vals, b_indptr, b_indices, b_vals, cp, c_indices, c_vals, bitmaps, L, dense_ws, dense_slots, n, hdr, st);
-    return run_classes<float, int64_t, true>(pr.sm_count, counts, offs, perm, a_indptr, a_indices, a_vals, b_indptr, b_indices, b_vals, cp, c_indices, c_vals, bitmaps, L, dense_ws, dense_slots, n, hdr, st);
-  }
-  if (pt == B2S_I32) return run_classes<double, int32_t, true>(pr.sm_count, counts, offs, perm, a_indptr, a_indices, a_vals, b_indptr, b_indices, b_vals, cp, c_indices, c_vals, bitmaps, L, dense_ws, dense_slots, n, hdr, st);
-  return run_classes<double, int64_t, true>(pr.sm_count, counts, offs, perm, a_indptr, a_indices, a_vals, b_indptr, b_indices, b_vals, cp, c_indices, c_vals, bitmaps, L, dense_ws, dense_slots, n, hdr, st);
+  return with_value_type(vt, [&](auto v) {
+    return with_index_type(pt, [&](auto p) {
+      return run_classes<decltype(v), decltype(p), true>(pr.sm_count, counts, offs, perm, a_indptr, a_indices, a_vals,
+                                                         b_indptr, b_indices, b_vals, cp, c_indices, c_vals, bitmaps, L,
+                                                         dense_ws, dense_slots, n, hdr, st);
+    });
+  });
 }
 
 }  // extern "C"

@@ -435,15 +435,6 @@ static int spmm_vec(int64_t nrows, int64_t nnz, int64_t k, const void* indptr, c
   return launch_spmm<V, I, P, 1>(nrows, nnz, k, indptr, indices, vals, X, ldx, Y, ldy, st);
 }
 
-template <typename V>
-static int spmm_idx(int it, int pt, int64_t nrows, int64_t nnz, int64_t k, const void* indptr, const void* indices, const void* vals,
-                    const void* X, int64_t ldx, void* Y, int64_t ldy, cudaStream_t st) {
-  if (it == B2S_I32 && pt == B2S_I32) return spmm_vec<V, int32_t, int32_t>(nrows, nnz, k, indptr, indices, vals, X, ldx, Y, ldy, st);
-  if (it == B2S_I32 && pt == B2S_I64) return spmm_vec<V, int32_t, int64_t>(nrows, nnz, k, indptr, indices, vals, X, ldx, Y, ldy, st);
-  if (it == B2S_I64 && pt == B2S_I32) return spmm_vec<V, int64_t, int32_t>(nrows, nnz, k, indptr, indices, vals, X, ldx, Y, ldy, st);
-  return spmm_vec<V, int64_t, int64_t>(nrows, nnz, k, indptr, indices, vals, X, ldx, Y, ldy, st);
-}
-
 }  // namespace b2s
 
 using namespace b2s;
@@ -476,8 +467,11 @@ int b2s_spmm_csr(int vt, int it, int pt, int64_t nrows, int64_t ncols, int64_t n
   B2S_CHECK_ARG(ncols == 0 || nnz == 0 || X != nullptr, "X is NULL");
   B2S_CHECK_ARG(Y != nullptr, "Y is NULL");
   cudaStream_t st = (cudaStream_t)stream;
-  if (vt == B2S_F32) return spmm_idx<float>(it, pt, nrows, nnz, k, indptr, indices, vals, X, ldx, Y, ldy, st);
-  return spmm_idx<double>(it, pt, nrows, nnz, k, indptr, indices, vals, X, ldx, Y, ldy, st);
+  return with_value_type(vt, [&](auto v) {
+    return with_index_types(it, pt, [&](auto i, auto p) {
+      return spmm_vec<decltype(v), decltype(i), decltype(p)>(nrows, nnz, k, indptr, indices, vals, X, ldx, Y, ldy, st);
+    });
+  });
 }
 
 }  // extern "C"

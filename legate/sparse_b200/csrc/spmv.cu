@@ -217,79 +217,13 @@ static int launch_pack(int it, int pt, const void* indptr, const void* indices, 
   uint16_t* r = const_cast<uint16_t*>(pk.rows);
   long long* b = const_cast<long long*>(pk.base);
   const int vb = pk.vb;
-  if (it == B2S_I32 && pt == B2S_I32)
-    spmv_pack_kernel<int32_t, int32_t, WRITE><<<grid, 256, 0, st>>>((const int32_t*)indptr, (const int32_t*)indices, plan, ntiles, c, r, b, stat, vals, vbytes, vb, dict);
-  else if (it == B2S_I32)
-    spmv_pack_kernel<int32_t, int64_t, WRITE><<<grid, 256, 0, st>>>((const int64_t*)indptr, (const int32_t*)indices, plan, ntiles, c, r, b, stat, vals, vbytes, vb, dict);
-  else if (pt == B2S_I32)
-    spmv_pack_kernel<int64_t, int32_t, WRITE><<<grid, 256, 0, st>>>((const int32_t*)indptr, (const int64_t*)indices, plan, ntiles, c, r, b, stat, vals, vbytes, vb, dict);
-  else
-    spmv_pack_kernel<int64_t, int64_t, WRITE><<<grid, 256, 0, st>>>((const int64_t*)indptr, (const int64_t*)indices, plan, ntiles, c, r, b, stat, vals, vbytes, vb, dict);
-  B2S_LAUNCH_CHECK();
-  return B2S_OK;
-}
-
-// Distinct bit patterns of vals[0, n), per block: each block keeps up to kMaxDict + 1 of them in shared memory (the
-// one past kMaxDict only marks the overflow, after which the block stops) and writes them to tabs[block], their count
-// to counts[block].  A warp looks its values up in the table and, for the ones it misses, inserts them in turn under a
-// block lock held by lane 0.  The host merges the blocks' tables (dict_collect).
-constexpr int kDictBlocks = 1024;
-template <typename U>
-__global__ void __launch_bounds__(256)
-spmv_dict_kernel(const U* __restrict__ vals, int64_t n, unsigned long long* __restrict__ tabs, int* __restrict__ counts) {
-  constexpr int CAP = kMaxDict + 1;
-  __shared__ U tab[CAP];
-  __shared__ int cnt, lock;
-  if (threadIdx.x == 0) { cnt = 0; lock = 0; }
-  __syncthreads();
-  volatile U* vtab = tab;
-  volatile int* vcnt = &cnt;
-  const unsigned full = 0xffffffffu;
-  const int lane = threadIdx.x & 31;
-  const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
-  for (int64_t base = warp * 128; base < n; base += nwarps * 128) {      // warp-uniform
-    if (__shfl_sync(full, *vcnt, 0) > kMaxDict) break;
-    U v[4];
-    bool in[4];
-#pragma unroll
-    for (int q = 0; q < 4; q++) {
-      const int64_t k = base + 32 * q + lane;
-      in[q] = k < n;
-      v[q] = in[q] ? vals[k] : (U)0;
-    }
-#pragma unroll
-    for (int q = 0; q < 4; q++) {
-      const int c = *vcnt;
-      bool hit = !in[q];
-      for (int i = 0; i < c && i < CAP && !hit; i++) hit = vtab[i] == v[q];
-      unsigned miss = __ballot_sync(full, !hit);
-      if (!miss) continue;
-      if (lane == 0) while (atomicCAS(&lock, 0, 1) != 0) {}
-      __syncwarp();
-      __threadfence_block();
-      while (miss) {
-        const U cand = __shfl_sync(full, v[q], __ffs(miss) - 1);
-        const int c2 = *vcnt;
-        bool found = false;
-        for (int i = 0; i < c2 && i < CAP; i++) found = found || vtab[i] == cand;
-        if (lane == 0 && !found && c2 < CAP) {
-          vtab[c2] = cand;
-          __threadfence_block();
-          *vcnt = c2 + 1;
-        }
-        __syncwarp();
-        miss &= ~__ballot_sync(full, in[q] && v[q] == cand);
-      }
-      __threadfence_block();
-      __syncwarp();
-      if (lane == 0) atomicExch(&lock, 0);
-    }
-  }
-  __syncthreads();
-  const int c = cnt < CAP ? cnt : CAP;
-  if ((int)threadIdx.x < c) tabs[(int64_t)blockIdx.x * CAP + threadIdx.x] = (unsigned long long)tab[threadIdx.x];
-  if (threadIdx.x == 0) counts[blockIdx.x] = cnt;
+  return with_index_types(it, pt, [&](auto i, auto p) {
+    using I = decltype(i); using P = decltype(p);
+    spmv_pack_kernel<I, P, WRITE><<<grid, 256, 0, st>>>((const P*)indptr, (const I*)indices, plan, ntiles, c, r, b, stat,
+                                                        vals, vbytes, vb, dict);
+    B2S_LAUNCH_CHECK();
+    return B2S_OK;
+  });
 }
 
 // ---- row templates (TemplateTable) ------------------------------------------------------------------------------
@@ -320,22 +254,46 @@ __device__ __forceinline__ bool tpl_row_hash(const P* __restrict__ indptr, const
   return true;
 }
 
-// Pass 1: the distinct signature hashes of the rows, per block, with one representative row each -- modelled on
-// spmv_dict_kernel (a bounded shared table, misses inserted under a block lock).  counts[block] > kMaxTemplates: the
-// block saw more signatures than that, or a row that cannot be a template.
-constexpr int kTplBlocks = 1024;
+// Keys of the distinct-key pass (distinct_keys_kernel): key(item, &k) stores the key of one item, or returns false for
+// an item that cannot be keyed.
+// The value dictionary: a nonzero's value bit pattern (fp32 zero-extended).
+struct ValueBitsKey {
+  const void* vals;
+  int vbytes;
+  __device__ __forceinline__ bool operator()(long long k, unsigned long long* key) const {
+    *key = tpl_bits(vals, vbytes, k);
+    return true;
+  }
+};
+// Row templates: a row's signature hash.
 template <typename I, typename P>
+struct RowSignatureKey {
+  const P* indptr;
+  const I* indices;
+  const void* vals;
+  int vbytes;
+  __device__ __forceinline__ bool operator()(long long r, unsigned long long* key) const {
+    return tpl_row_hash(indptr, indices, vals, vbytes, r, key);
+  }
+};
+
+// The distinct keys of items [0, n), per block: each block keeps up to CAP + 1 of them in shared memory, with the
+// first item it saw under each (the entry past CAP only marks the overflow, after which the block stops), and writes
+// them to keys / reps[block * (CAP + 1) ...], their count to counts[block]; an item that cannot be keyed stops the
+// block with the count CAP + 1 too.  A warp looks its keys up in the table and, for the ones it misses, inserts them
+// in turn under a block lock held by lane 0.  The host merges the blocks' tables (distinct_keys).
+constexpr int kKeyBlocks = 1024;
+template <int CAP, typename Key>
 __global__ void __launch_bounds__(256)
-tpl_collect_kernel(int64_t nrows, const P* __restrict__ indptr, const I* __restrict__ indices,
-                   const void* __restrict__ vals, int vbytes, unsigned long long* __restrict__ tabs,
-                   long long* __restrict__ reps, int* __restrict__ counts) {
-  constexpr int CAP = kMaxTemplates + 1;
-  __shared__ unsigned long long th[CAP];
-  __shared__ long long tr[CAP];
+distinct_keys_kernel(int64_t n, Key key, unsigned long long* __restrict__ keys, long long* __restrict__ reps,
+                     int* __restrict__ counts) {
+  constexpr int TAB = CAP + 1;
+  __shared__ unsigned long long tk[TAB];
+  __shared__ long long tr[TAB];
   __shared__ int cnt, lock, bad;
   if (threadIdx.x == 0) { cnt = 0; lock = 0; bad = 0; }
   __syncthreads();
-  volatile unsigned long long* vth = th;
+  volatile unsigned long long* vtk = tk;
   volatile long long* vtr = tr;
   volatile int* vcnt = &cnt;
   volatile int* vbad = &bad;
@@ -343,47 +301,54 @@ tpl_collect_kernel(int64_t nrows, const P* __restrict__ indptr, const I* __restr
   const int lane = threadIdx.x & 31;
   const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
-  for (int64_t base = warp * 32; base < nrows; base += nwarps * 32) {      // warp-uniform
-    if (__shfl_sync(full, (*vcnt > kMaxTemplates || *vbad) ? 1 : 0, 0)) break;
-    const long long r = base + lane;
-    unsigned long long h = 0;
-    bool in = r < nrows;
-    if (in && !tpl_row_hash(indptr, indices, vals, vbytes, r, &h)) { *vbad = 1; in = false; }
-    const int c = *vcnt;
-    bool hit = !in;
-    for (int i = 0; i < c && i < CAP && !hit; i++) hit = vth[i] == h;
-    unsigned miss = __ballot_sync(full, !hit);
-    if (!miss) continue;
-    if (lane == 0) while (atomicCAS(&lock, 0, 1) != 0) {}
-    __syncwarp();
-    __threadfence_block();
-    while (miss) {
-      const int src = __ffs(miss) - 1;
-      const unsigned long long cand = __shfl_sync(full, h, src);
-      const long long crow = __shfl_sync(full, r, src);
-      const int c2 = *vcnt;
-      bool found = false;
-      for (int i = 0; i < c2 && i < CAP; i++) found = found || vth[i] == cand;
-      if (lane == 0 && !found && c2 < CAP) {
-        vth[c2] = cand;
-        vtr[c2] = crow;
-        __threadfence_block();
-        *vcnt = c2 + 1;
-      }
-      __syncwarp();
-      miss &= ~__ballot_sync(full, in && h == cand);
+  for (int64_t base = warp * 128; base < n; base += nwarps * 128) {      // warp-uniform
+    if (__shfl_sync(full, (*vcnt > CAP || *vbad) ? 1 : 0, 0)) break;
+    unsigned long long k[4];
+    bool in[4];
+#pragma unroll
+    for (int q = 0; q < 4; q++) {
+      const long long i = base + 32 * q + lane;
+      k[q] = 0;
+      in[q] = i < n;
+      if (in[q] && !key(i, &k[q])) { *vbad = 1; in[q] = false; }
     }
-    __threadfence_block();
-    __syncwarp();
-    if (lane == 0) atomicExch(&lock, 0);
+#pragma unroll
+    for (int q = 0; q < 4; q++) {
+      const int c = *vcnt;
+      bool hit = !in[q];
+      for (int j = 0; j < c && j < TAB && !hit; j++) hit = vtk[j] == k[q];
+      unsigned miss = __ballot_sync(full, !hit);
+      if (!miss) continue;
+      if (lane == 0) while (atomicCAS(&lock, 0, 1) != 0) {}
+      __syncwarp();
+      __threadfence_block();
+      while (miss) {
+        const int src = __ffs(miss) - 1;
+        const unsigned long long cand = __shfl_sync(full, k[q], src);
+        const int c2 = *vcnt;
+        bool found = false;
+        for (int j = 0; j < c2 && j < TAB; j++) found = found || vtk[j] == cand;
+        if (lane == 0 && !found && c2 < TAB) {
+          vtk[c2] = cand;
+          vtr[c2] = base + 32 * q + src;
+          __threadfence_block();
+          *vcnt = c2 + 1;
+        }
+        __syncwarp();
+        miss &= ~__ballot_sync(full, in[q] && k[q] == cand);
+      }
+      __threadfence_block();
+      __syncwarp();
+      if (lane == 0) atomicExch(&lock, 0);
+    }
   }
   __syncthreads();
-  const int c = cnt < CAP ? cnt : CAP;
+  const int c = cnt < TAB ? cnt : TAB;
   if ((int)threadIdx.x < c) {
-    tabs[(int64_t)blockIdx.x * CAP + threadIdx.x] = th[threadIdx.x];
-    reps[(int64_t)blockIdx.x * CAP + threadIdx.x] = tr[threadIdx.x];
+    keys[(int64_t)blockIdx.x * TAB + threadIdx.x] = tk[threadIdx.x];
+    reps[(int64_t)blockIdx.x * TAB + threadIdx.x] = tr[threadIdx.x];
   }
-  if (threadIdx.x == 0) counts[blockIdx.x] = bad ? CAP + 1 : cnt;
+  if (threadIdx.x == 0) counts[blockIdx.x] = bad ? TAB : cnt;
 }
 
 // The table from the representative rows reps[0, n) (one thread per template; hashes ascending)
@@ -482,6 +447,100 @@ static int64_t tiles_for(int cfg, int vt, int64_t nrows, int64_t nnz) {
   return (nrows + nnz + T - 1) / T;
 }
 
+// The distinct keys of items [0, n) under `key`, ascending, each with its smallest representative item, into *out;
+// *fits = false when there are more than CAP of them or an item cannot be keyed.  One pass over the items; the
+// per-block tables come back to the host (at most kKeyBlocks x (CAP + 1) entries) and are merged there.  One host sync.
+template <int CAP, typename Key>
+static int distinct_keys(int64_t n, const Key& key, cudaStream_t st,
+                         std::vector<std::pair<unsigned long long, long long>>* out, bool* fits) {
+  constexpr int TAB = CAP + 1;
+  *fits = false;
+  out->clear();
+  const int64_t blocks64 = (n + 1023) / 1024;
+  const int blocks = (int)(blocks64 < kKeyBlocks ? blocks64 : kKeyBlocks);
+  if (blocks <= 0) { *fits = true; return B2S_OK; }
+  unsigned char* tmp = nullptr;
+  const size_t tab_b = sizeof(unsigned long long) * TAB * (size_t)blocks;
+  B2S_CUDA(cudaMallocAsync((void**)&tmp, 2 * tab_b + sizeof(int) * (size_t)blocks, st));
+  unsigned long long* keys = (unsigned long long*)tmp;
+  long long* reps = (long long*)(tmp + tab_b);
+  int* counts = (int*)(tmp + 2 * tab_b);
+  distinct_keys_kernel<CAP><<<blocks, 256, 0, st>>>(n, key, keys, reps, counts);
+  cudaError_t le = cudaGetLastError();
+  std::vector<unsigned long long> host_keys((size_t)TAB * blocks);
+  std::vector<long long> host_reps((size_t)TAB * blocks);
+  std::vector<int> host_counts(blocks);
+  if (le == cudaSuccess) le = cudaMemcpyAsync(host_keys.data(), keys, tab_b, cudaMemcpyDeviceToHost, st);
+  if (le == cudaSuccess) le = cudaMemcpyAsync(host_reps.data(), reps, tab_b, cudaMemcpyDeviceToHost, st);
+  if (le == cudaSuccess) le = cudaMemcpyAsync(host_counts.data(), counts, sizeof(int) * blocks, cudaMemcpyDeviceToHost, st);
+  if (le == cudaSuccess) le = cudaStreamSynchronize(st);
+  cudaFreeAsync(tmp, st);
+  B2S_CUDA(le);
+  for (int b = 0; b < blocks; b++) {
+    if (host_counts[b] > CAP) { out->clear(); return B2S_OK; }
+    for (int i = 0; i < host_counts[b]; i++)
+      out->emplace_back(host_keys[(size_t)TAB * b + i], host_reps[(size_t)TAB * b + i]);
+  }
+  // sorted by (key, item): unique keeps each key's smallest item
+  std::sort(out->begin(), out->end());
+  out->erase(std::unique(out->begin(), out->end(), [](const auto& a, const auto& b) { return a.first == b.first; }),
+             out->end());
+  if (out->size() > (size_t)CAP) { out->clear(); return B2S_OK; }
+  *fits = true;
+  return B2S_OK;
+}
+
+// b2s_spmv_plan_templates for column index type I and row pointer type P
+template <typename I, typename P>
+static int plan_templates(PlanHandle* h, const P* indptr, const I* indices, const void* vals, void* buf_dev,
+                          cudaStream_t st) {
+  const int vbytes = h->vt == B2S_F32 ? 4 : 8;
+  const int64_t nrows = h->nrows;
+  // pass 1: the distinct signature hashes, ascending (so ids do not depend on the run), with a representative row each
+  std::vector<std::pair<unsigned long long, long long>> sigs;
+  bool fits = false;
+  if (int rc = distinct_keys<kMaxTemplates>(nrows, RowSignatureKey<I, P>{indptr, indices, vals, vbytes}, st, &sigs,
+                                            &fits))
+    return rc;
+  const int n = (int)sigs.size();
+  if (!fits || n == 0) return B2S_OK;
+  // the table from the representative rows, then pass 2: every row compared with its template
+  long long reps_host[kMaxTemplates];
+  for (int i = 0; i < n; i++) reps_host[i] = sigs[i].second;
+  TemplateTable* tab = (TemplateTable*)buf_dev;
+  uint8_t* ids = (uint8_t*)buf_dev + kTplIdsOff;
+  int lens[kMaxTemplates + 1] = {0};   // lengths, then the bad flag
+  // scratch: the representative rows, then the bad flag
+  unsigned char* tmp = nullptr;
+  B2S_CUDA(cudaMallocAsync((void**)&tmp, sizeof(long long) * kMaxTemplates + 16, st));
+  long long* reps = (long long*)tmp;
+  int* bad = (int*)(tmp + sizeof(long long) * kMaxTemplates);
+  cudaError_t le = cudaMemsetAsync(buf_dev, 0, sizeof(TemplateTable), st);
+  if (le == cudaSuccess) le = cudaMemsetAsync(bad, 0, sizeof(int), st);
+  if (le == cudaSuccess) le = cudaMemcpyAsync(reps, reps_host, sizeof(long long) * n, cudaMemcpyHostToDevice, st);
+  if (le == cudaSuccess) {
+    tpl_table_kernel<I, P><<<1, 32, 0, st>>>(indptr, indices, vals, vbytes, reps, n, tab);
+    tpl_assign_kernel<I, P><<<(unsigned)((nrows + 255) / 256), 256, 0, st>>>(nrows, indptr, indices, vals, vbytes, tab, n,
+                                                                             ids, bad);
+    le = cudaGetLastError();
+  }
+  const int* dev_lens = (const int*)((const unsigned char*)buf_dev + offsetof(TemplateTable, len));
+  if (le == cudaSuccess) le = cudaMemcpyAsync(lens, dev_lens, sizeof(int) * kMaxTemplates, cudaMemcpyDeviceToHost, st);
+  if (le == cudaSuccess) le = cudaMemcpyAsync(lens + kMaxTemplates, bad, sizeof(int), cudaMemcpyDeviceToHost, st);
+  if (le == cudaSuccess) le = cudaStreamSynchronize(st);
+  cudaFreeAsync(tmp, st);
+  B2S_CUDA(le);
+  if (lens[kMaxTemplates]) return B2S_OK;
+  int maxlen = 0;
+  for (int i = 0; i < n; i++) maxlen = lens[i] > maxlen ? lens[i] : maxlen;
+  h->tpl = tab;
+  h->tpl_vals = vals;
+  h->ntpl = n;
+  h->tpl_maxlen = maxlen;
+  h->use_tpl = 1;
+  return B2S_OK;
+}
+
 }  // namespace b2s
 
 using namespace b2s;
@@ -535,9 +594,13 @@ static int plan_create_impl(int vt, int it, int pt, int64_t nrows, int64_t ncols
     B2S_CUDA(cudaMemsetAsync(stat, 0, 16, st));
     const unsigned g2 = (unsigned)((ns * 32 + 255) / 256);
     const int shift = vt == B2S_F32 ? 2 : 3;
-    if (it == B2S_I32) spmv_locality_kernel<int32_t><<<g2, 256, 0, st>>>(nnz, (const int32_t*)indices, shift, ns, stat);
-    else               spmv_locality_kernel<int64_t><<<g2, 256, 0, st>>>(nnz, (const int64_t*)indices, shift, ns, stat);
-    B2S_LAUNCH_CHECK();
+    if (int rc = with_index_type(it, [&](auto i) {
+          using I = decltype(i);
+          spmv_locality_kernel<I><<<g2, 256, 0, st>>>(nnz, (const I*)indices, shift, ns, stat);
+          B2S_LAUNCH_CHECK();
+          return B2S_OK;
+        }))
+      return rc;
     unsigned long long total = 0;
     B2S_CUDA(cudaMemcpyAsync(&total, stat, sizeof(total), cudaMemcpyDeviceToHost, st));
     B2S_CUDA(cudaStreamSynchronize(st));
@@ -555,16 +618,18 @@ static int plan_create_impl(int vt, int it, int pt, int64_t nrows, int64_t ncols
   // 2. tile boundaries + row-shape codes for the chosen tile shape
   if (ntiles > 0) {
     const int64_t T = cfg_T(cfg, vt);
-    const unsigned grid = (unsigned)((ntiles + 1 + 255) / 256);
-    if (pt == B2S_I32) spmv_plan_kernel<int32_t><<<grid, 256, 0, st>>>(nrows, (const int32_t*)indptr, T, ntiles, dev);
-    else               spmv_plan_kernel<int64_t><<<grid, 256, 0, st>>>(nrows, (const int64_t*)indptr, T, ntiles, dev);
-    B2S_LAUNCH_CHECK();
-    B2S_CUDA(cudaMemsetAsync(stat, 0, 16, st));
-    const unsigned gu = (unsigned)((ntiles + 255) / 256);
+    const unsigned grid = (unsigned)((ntiles + 1 + 255) / 256), gu = (unsigned)((ntiles + 255) / 256);
     const int ept = vt == B2S_F32 ? 4 : 2;
-    if (pt == B2S_I32) spmv_plan_shape_kernel<int32_t><<<gu, 256, 0, st>>>((const int32_t*)indptr, ntiles, dev, ept, stat);
-    else               spmv_plan_shape_kernel<int64_t><<<gu, 256, 0, st>>>((const int64_t*)indptr, ntiles, dev, ept, stat);
-    B2S_LAUNCH_CHECK();
+    if (int rc = with_index_type(pt, [&](auto p) {
+          using P = decltype(p);
+          spmv_plan_kernel<P><<<grid, 256, 0, st>>>(nrows, (const P*)indptr, T, ntiles, dev);
+          B2S_LAUNCH_CHECK();
+          B2S_CUDA(cudaMemsetAsync(stat, 0, 16, st));
+          spmv_plan_shape_kernel<P><<<gu, 256, 0, st>>>((const P*)indptr, ntiles, dev, ept, stat);
+          B2S_LAUNCH_CHECK();
+          return B2S_OK;
+        }))
+      return rc;
     unsigned long long ut[2] = {0, 0};
     B2S_CUDA(cudaMemcpyAsync(ut, stat, sizeof(ut), cudaMemcpyDeviceToHost, st));
     B2S_CUDA(cudaStreamSynchronize(st));
@@ -632,9 +697,13 @@ static int plan_create_impl(int vt, int it, int pt, int64_t nrows, int64_t ncols
     B2S_CUDA(cudaMemcpyAsync(dtmp, kb_host, sizeof(long long) * (K + 1), cudaMemcpyHostToDevice, st));
     B2S_CUDA(cudaMemcpyAsync(dtmp + K + 1, mm_host, sizeof(long long) * 2 * K, cudaMemcpyHostToDevice, st));
     const int bpc = 64;
-    if (it == B2S_I32) spmv_col_window_kernel<int32_t><<<K * bpc, 256, 0, st>>>((const int32_t*)indices, dtmp, K, bpc, dtmp + K + 1);
-    else               spmv_col_window_kernel<int64_t><<<K * bpc, 256, 0, st>>>((const int64_t*)indices, dtmp, K, bpc, dtmp + K + 1);
-    B2S_LAUNCH_CHECK();
+    if (int rc = with_index_type(it, [&](auto i) {
+          using I = decltype(i);
+          spmv_col_window_kernel<I><<<K * bpc, 256, 0, st>>>((const I*)indices, dtmp, K, bpc, dtmp + K + 1);
+          B2S_LAUNCH_CHECK();
+          return B2S_OK;
+        }))
+      return rc;
     B2S_CUDA(cudaMemcpyAsync(mm_host, dtmp + K + 1, sizeof(long long) * 2 * K, cudaMemcpyDeviceToHost, st));
     B2S_CUDA(cudaStreamSynchronize(st));
     B2S_CUDA(cudaFreeAsync(dtmp, st));
@@ -692,44 +761,6 @@ int64_t b2s_spmv_plan_pack_bytes(const void* plan) {
   return b + c + r + kDictBytes;
 }
 
-// The sorted distinct bit patterns of vals[0, nnz) into *d; false when there are more than kMaxDict.  One pass over
-// the values; the per-block tables come back to the host (at most kDictBlocks x 17 patterns) and are merged there.
-static int dict_collect(int vt, int64_t nnz, const void* vals, cudaStream_t st, DictBits* d, bool* fits) {
-  constexpr int CAP = kMaxDict + 1;
-  *fits = false;
-  d->n = 0;
-  const int64_t blocks64 = (nnz + 1023) / 1024;
-  const int blocks = (int)(blocks64 < kDictBlocks ? blocks64 : kDictBlocks);
-  if (blocks <= 0) return B2S_OK;
-  unsigned char* tmp = nullptr;
-  const size_t tab_b = sizeof(unsigned long long) * CAP * (size_t)blocks;
-  B2S_CUDA(cudaMallocAsync((void**)&tmp, tab_b + sizeof(int) * (size_t)blocks, st));
-  unsigned long long* tabs = (unsigned long long*)tmp;
-  int* counts = (int*)(tmp + tab_b);
-  if (vt == B2S_F64) spmv_dict_kernel<unsigned long long><<<blocks, 256, 0, st>>>((const unsigned long long*)vals, nnz, tabs, counts);
-  else               spmv_dict_kernel<unsigned><<<blocks, 256, 0, st>>>((const unsigned*)vals, nnz, tabs, counts);
-  cudaError_t le = cudaGetLastError();
-  std::vector<unsigned long long> host_tabs((size_t)CAP * blocks);
-  std::vector<int> host_counts(blocks);
-  if (le == cudaSuccess) le = cudaMemcpyAsync(host_tabs.data(), tabs, tab_b, cudaMemcpyDeviceToHost, st);
-  if (le == cudaSuccess) le = cudaMemcpyAsync(host_counts.data(), counts, sizeof(int) * blocks, cudaMemcpyDeviceToHost, st);
-  if (le == cudaSuccess) le = cudaStreamSynchronize(st);
-  cudaFreeAsync(tmp, st);
-  B2S_CUDA(le);
-  std::vector<unsigned long long> all;
-  for (int b = 0; b < blocks; b++) {
-    if (host_counts[b] > kMaxDict) return B2S_OK;
-    all.insert(all.end(), host_tabs.begin() + (size_t)CAP * b, host_tabs.begin() + (size_t)CAP * b + host_counts[b]);
-  }
-  std::sort(all.begin(), all.end());
-  all.erase(std::unique(all.begin(), all.end()), all.end());
-  if (all.size() > (size_t)kMaxDict) return B2S_OK;
-  for (size_t i = 0; i < all.size(); i++) d->v[i] = all[i];
-  d->n = (int)all.size();
-  *fits = true;
-  return B2S_OK;
-}
-
 // Fills the packed buffer (coded when vals != NULL, see PackedTiles) and switches the plan's launches to it.
 static int pack_write(PlanHandle* h, const void* indptr, const void* indices, const void* vals, int vb,
                       const DictBits& dict, void* buf_dev, cudaStream_t st) {
@@ -783,9 +814,13 @@ int b2s_spmv_plan_pack_coded(void* plan, const void* indptr, const void* indices
   if (int rc = pack_check(h, indptr, indices, buf_dev)) return rc;
   B2S_CHECK_ARG(vals != nullptr, "vals is NULL");
   cudaStream_t st = (cudaStream_t)stream;
-  DictBits d{};
+  // the dictionary: the sorted distinct bit patterns, so a value's code is its pattern's rank
+  std::vector<std::pair<unsigned long long, long long>> bits;
   bool fits = false;
-  if (int rc = dict_collect(h->vt, h->nnz, vals, st, &d, &fits)) return rc;
+  if (int rc = distinct_keys<kMaxDict>(h->nnz, ValueBitsKey{vals, h->vt == B2S_F32 ? 4 : 8}, st, &bits, &fits)) return rc;
+  DictBits d{};
+  d.n = (int)bits.size();
+  for (int i = 0; i < d.n; i++) d.v[i] = bits[i].first;
   int vb = 0;
   while ((1 << vb) < d.n) vb++;
   const bool coded = fits && h->pack_w < (1LL << (16 - vb));
@@ -813,95 +848,10 @@ int b2s_spmv_plan_templates(void* plan, const void* indptr, const void* indices,
   B2S_CHECK_ARG(indptr && indices && vals, "indptr / indices / vals is NULL");
   B2S_CHECK_ARG(buf_dev != nullptr && aligned16(buf_dev), "template buffer must be non-NULL and 16-byte aligned");
   B2S_CHECK_ARG(h->tpl == nullptr, "the plan already has row templates");
-  constexpr int CAP = kMaxTemplates + 1;
-  cudaStream_t st = (cudaStream_t)stream;
-  const int vbytes = h->vt == B2S_F32 ? 4 : 8;
-  const int64_t nrows = h->nrows;
-  const int64_t blocks64 = (nrows + 255) / 256;
-  const int blocks = (int)(blocks64 < kTplBlocks ? blocks64 : kTplBlocks);
-  // scratch: per-block hashes + representative rows + counts, then the merged representatives and the bad flag
-  const size_t tab_b = sizeof(unsigned long long) * CAP * (size_t)blocks;
-  const size_t cnt_off = 2 * tab_b, reps_off = round16(cnt_off + sizeof(int) * (size_t)blocks);
-  const size_t bad_off = reps_off + sizeof(long long) * kMaxTemplates;
-  unsigned char* tmp = nullptr;
-  B2S_CUDA(cudaMallocAsync((void**)&tmp, bad_off + 16, st));
-  unsigned long long* tabs = (unsigned long long*)tmp;
-  long long* breps = (long long*)(tmp + tab_b);
-  int* counts = (int*)(tmp + cnt_off);
-  long long* reps = (long long*)(tmp + reps_off);
-  int* bad = (int*)(tmp + bad_off);
-  const int it = h->it, pt = h->pt;
-#define B2S_TPL_LAUNCH(KERNEL, GRID, BLOCK, ...)                                                                      \
-  do {                                                                                                               \
-    if (it == B2S_I32 && pt == B2S_I32)                                                                              \
-      KERNEL<int32_t, int32_t><<<GRID, BLOCK, 0, st>>>(nrows, (const int32_t*)indptr, (const int32_t*)indices, __VA_ARGS__); \
-    else if (it == B2S_I32)                                                                                          \
-      KERNEL<int32_t, int64_t><<<GRID, BLOCK, 0, st>>>(nrows, (const int64_t*)indptr, (const int32_t*)indices, __VA_ARGS__); \
-    else if (pt == B2S_I32)                                                                                          \
-      KERNEL<int64_t, int32_t><<<GRID, BLOCK, 0, st>>>(nrows, (const int32_t*)indptr, (const int64_t*)indices, __VA_ARGS__); \
-    else                                                                                                             \
-      KERNEL<int64_t, int64_t><<<GRID, BLOCK, 0, st>>>(nrows, (const int64_t*)indptr, (const int64_t*)indices, __VA_ARGS__); \
-  } while (0)
-  // pass 1: per-block signature hashes, merged on the host
-  B2S_TPL_LAUNCH(tpl_collect_kernel, blocks, 256, vals, vbytes, tabs, breps, counts);
-  cudaError_t le = cudaGetLastError();
-  std::vector<unsigned long long> host_tabs((size_t)CAP * blocks);
-  std::vector<long long> host_reps((size_t)CAP * blocks);
-  std::vector<int> host_counts(blocks);
-  if (le == cudaSuccess) le = cudaMemcpyAsync(host_tabs.data(), tabs, tab_b, cudaMemcpyDeviceToHost, st);
-  if (le == cudaSuccess) le = cudaMemcpyAsync(host_reps.data(), breps, tab_b, cudaMemcpyDeviceToHost, st);
-  if (le == cudaSuccess) le = cudaMemcpyAsync(host_counts.data(), counts, sizeof(int) * blocks, cudaMemcpyDeviceToHost, st);
-  if (le == cudaSuccess) le = cudaStreamSynchronize(st);
-  if (le != cudaSuccess) { cudaFreeAsync(tmp, st); B2S_CUDA(le); }
-  std::vector<std::pair<unsigned long long, long long>> all;   // (hash, smallest representative row)
-  bool fits = true;
-  for (int b = 0; b < blocks && fits; b++) {
-    if (host_counts[b] > kMaxTemplates) fits = false;
-    for (int i = 0; fits && i < host_counts[b]; i++)
-      all.emplace_back(host_tabs[(size_t)CAP * b + i], host_reps[(size_t)CAP * b + i]);
-  }
-  std::sort(all.begin(), all.end());
-  all.erase(std::unique(all.begin(), all.end(), [](const auto& a, const auto& b) { return a.first == b.first; }),
-            all.end());
-  const int n = (int)all.size();
-  if (!fits || n == 0 || n > kMaxTemplates) { B2S_CUDA(cudaFreeAsync(tmp, st)); return B2S_OK; }
-  // the table from the representative rows, then pass 2: every row compared with its template
-  long long reps_host[kMaxTemplates];
-  for (int i = 0; i < n; i++) reps_host[i] = all[i].second;
-  TemplateTable* tab = (TemplateTable*)buf_dev;
-  uint8_t* ids = (uint8_t*)buf_dev + kTplIdsOff;
-  int lens[kMaxTemplates + 1] = {0};   // lengths, then the bad flag
-  le = cudaMemsetAsync(buf_dev, 0, sizeof(TemplateTable), st);
-  if (le == cudaSuccess) le = cudaMemsetAsync(bad, 0, sizeof(int), st);
-  if (le == cudaSuccess) le = cudaMemcpyAsync(reps, reps_host, sizeof(long long) * n, cudaMemcpyHostToDevice, st);
-  if (le == cudaSuccess) {
-    if (it == B2S_I32 && pt == B2S_I32)
-      tpl_table_kernel<int32_t, int32_t><<<1, 32, 0, st>>>((const int32_t*)indptr, (const int32_t*)indices, vals, vbytes, reps, n, tab);
-    else if (it == B2S_I32)
-      tpl_table_kernel<int32_t, int64_t><<<1, 32, 0, st>>>((const int64_t*)indptr, (const int32_t*)indices, vals, vbytes, reps, n, tab);
-    else if (pt == B2S_I32)
-      tpl_table_kernel<int64_t, int32_t><<<1, 32, 0, st>>>((const int32_t*)indptr, (const int64_t*)indices, vals, vbytes, reps, n, tab);
-    else
-      tpl_table_kernel<int64_t, int64_t><<<1, 32, 0, st>>>((const int64_t*)indptr, (const int64_t*)indices, vals, vbytes, reps, n, tab);
-    B2S_TPL_LAUNCH(tpl_assign_kernel, (unsigned)((nrows + 255) / 256), 256, vals, vbytes, tab, n, ids, bad);
-    le = cudaGetLastError();
-  }
-#undef B2S_TPL_LAUNCH
-  const int* dev_lens = (const int*)((const unsigned char*)buf_dev + offsetof(TemplateTable, len));
-  if (le == cudaSuccess) le = cudaMemcpyAsync(lens, dev_lens, sizeof(int) * kMaxTemplates, cudaMemcpyDeviceToHost, st);
-  if (le == cudaSuccess) le = cudaMemcpyAsync(lens + kMaxTemplates, bad, sizeof(int), cudaMemcpyDeviceToHost, st);
-  if (le == cudaSuccess) le = cudaStreamSynchronize(st);
-  cudaFreeAsync(tmp, st);
-  B2S_CUDA(le);
-  if (lens[kMaxTemplates]) return B2S_OK;
-  int maxlen = 0;
-  for (int i = 0; i < n; i++) maxlen = lens[i] > maxlen ? lens[i] : maxlen;
-  h->tpl = tab;
-  h->tpl_vals = vals;
-  h->ntpl = n;
-  h->tpl_maxlen = maxlen;
-  h->use_tpl = 1;
-  return B2S_OK;
+  return with_index_types(h->it, h->pt, [&](auto i, auto p) {
+    using I = decltype(i); using P = decltype(p);
+    return plan_templates<I, P>(h, (const P*)indptr, (const I*)indices, vals, buf_dev, (cudaStream_t)stream);
+  });
 }
 
 /* tools / tests: 0 = launches stream the CSR arrays, 1 = the packed structure and the values, 2 = the packed structure

@@ -1123,12 +1123,9 @@ static int dispatch_cfg(int cfg, const SpmvArgs& a) {
 
 template <typename V, bool DOT>
 static int dispatch_idx(int it, int pt, int cfg, const SpmvArgs& a) {
-  if (it == B2S_I32 && pt == B2S_I32) return dispatch_cfg<V, int32_t, int32_t, DOT>(cfg, a);
-  if (it == B2S_I32 && pt == B2S_I64) return dispatch_cfg<V, int32_t, int64_t, DOT>(cfg, a);
-  if (it == B2S_I64 && pt == B2S_I32) return dispatch_cfg<V, int64_t, int32_t, DOT>(cfg, a);
-  if (it == B2S_I64 && pt == B2S_I64) return dispatch_cfg<V, int64_t, int64_t, DOT>(cfg, a);
-  set_error("bad index type codes it=%d pt=%d", it, pt);
-  return B2S_EINVAL;
+  return with_index_types(it, pt, [&](auto i, auto p) {
+    return dispatch_cfg<V, decltype(i), decltype(p), DOT>(cfg, a);
+  });
 }
 
 template <typename V, typename I, typename P>
@@ -1153,12 +1150,9 @@ static int launch_rowgroup(int64_t nrows, int64_t nnz, const void* indptr, const
 template <typename V>
 static int dispatch_rowgroup(int it, int pt, int64_t nrows, int64_t nnz, const void* indptr, const void* indices,
                              const void* vals, const void* x, void* y, cudaStream_t st) {
-  if (it == B2S_I32 && pt == B2S_I32) return launch_rowgroup<V, int32_t, int32_t>(nrows, nnz, indptr, indices, vals, x, y, st);
-  if (it == B2S_I32 && pt == B2S_I64) return launch_rowgroup<V, int32_t, int64_t>(nrows, nnz, indptr, indices, vals, x, y, st);
-  if (it == B2S_I64 && pt == B2S_I32) return launch_rowgroup<V, int64_t, int32_t>(nrows, nnz, indptr, indices, vals, x, y, st);
-  if (it == B2S_I64 && pt == B2S_I64) return launch_rowgroup<V, int64_t, int64_t>(nrows, nnz, indptr, indices, vals, x, y, st);
-  set_error("bad index type codes it=%d pt=%d", it, pt);
-  return B2S_EINVAL;
+  return with_index_types(it, pt, [&](auto i, auto p) {
+    return launch_rowgroup<V, decltype(i), decltype(p)>(nrows, nnz, indptr, indices, vals, x, y, st);
+  });
 }
 
 // Row-template launches: one resident wave of CTAs (occupancy x SMs) walking the row chunks in order.

@@ -185,14 +185,6 @@ csr_diagonal_kernel(int64_t nrows, const P* __restrict__ indptr, const I* __rest
   diag[i] = d;
 }
 
-template <typename V, typename I, typename P>
-static void launch_diag(int64_t nrows, const void* indptr, const void* indices, const void* vals, void* diag,
-                        cudaStream_t st) {
-  const unsigned grid = (unsigned)((nrows + VTHREADS - 1) / VTHREADS);
-  csr_diagonal_kernel<V, I, P><<<grid, VTHREADS, 0, st>>>(nrows, (const P*)indptr, (const I*)indices,
-                                                         (const V*)vals, (V*)diag);
-}
-
 static bool vec_aligned(const void* a, const void* b = nullptr, const void* c = nullptr, const void* d = nullptr) {
   return aligned16(a) && aligned16(b) && aligned16(c) && aligned16(d);
 }
@@ -275,17 +267,16 @@ int b2s_csr_diagonal(int vt, int it, int pt, int64_t nrows, const void* indptr, 
   if (nrows == 0) return B2S_OK;
   B2S_CHECK_ARG(indptr && diag_out, "NULL pointer");
   cudaStream_t st = (cudaStream_t)stream;
-#define B2S_DIAG(V)                                                                                   \
-  do {                                                                                                \
-    if (it == B2S_I32 && pt == B2S_I32) launch_diag<V, int32_t, int32_t>(nrows, indptr, indices, vals, diag_out, st); \
-    else if (it == B2S_I32) launch_diag<V, int32_t, int64_t>(nrows, indptr, indices, vals, diag_out, st);             \
-    else if (pt == B2S_I32) launch_diag<V, int64_t, int32_t>(nrows, indptr, indices, vals, diag_out, st);             \
-    else launch_diag<V, int64_t, int64_t>(nrows, indptr, indices, vals, diag_out, st);                                \
-  } while (0)
-  if (vt == B2S_F32) B2S_DIAG(float); else B2S_DIAG(double);
-#undef B2S_DIAG
-  B2S_LAUNCH_CHECK();
-  return B2S_OK;
+  const unsigned grid = (unsigned)((nrows + VTHREADS - 1) / VTHREADS);
+  return with_value_type(vt, [&](auto v) {
+    return with_index_types(it, pt, [&](auto i, auto p) {
+      using V = decltype(v); using I = decltype(i); using P = decltype(p);
+      csr_diagonal_kernel<V, I, P><<<grid, VTHREADS, 0, st>>>(nrows, (const P*)indptr, (const I*)indices, (const V*)vals,
+                                                             (V*)diag_out);
+      B2S_LAUNCH_CHECK();
+      return B2S_OK;
+    });
+  });
 }
 
 int b2s_copy(int vt, int64_t n, void* dst, const void* src, void* stream) {
