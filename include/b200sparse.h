@@ -376,6 +376,16 @@ int         b2s_csr_scale(int vt, int it, int pt, int64_t m, int64_t n, int64_t 
                           const void* indptr, const void* indices, const void* vals,
                           const void* d, int64_t ldd, void* out_vals, void* stream);
 
+/* ---- SDDMM: out[p] = vals[p] * sum_t C[i*ldc + t] * Dt[j*ldd + t] for every stored entry p = (i, j) of A ----------
+ * Replaces CSRSDDMM::gpu_variant (src/sparse/array/csr/sddmm.cu:27-105) and sddmm_impl (sparse/csr.py:1243-1314);
+ * CPU body sddmm.cc:25-48.  C is (nrows x k) and Dt is D transposed, (ncols x k), both row-major with row strides
+ * ldc, ldd >= k.  Every stored entry gets its own value (no merging of repeated columns, unsorted rows kept); k = 0
+ * gives vals[p] * 0.  Each dot product is summed in an order fixed by k and the operands' 16-byte alignment, so the
+ * result does not depend on the index widths.  No host sync, no allocation: capturable in a CUDA graph. */
+int         b2s_sddmm_csr(int vt, int it, int pt, int64_t nrows, int64_t ncols, int64_t nnz, int64_t k,
+                          const void* indptr, const void* indices, const void* vals,
+                          const void* C, int64_t ldc, const void* Dt, int64_t ldd, void* out, void* stream);
+
 /* ---- multi-GPU: NCCL communicator owned by the library (SURVEY 8b) -----------------------------------------
  * For hosts without torch.distributed (and for multi-node runs): the library binds NCCL at run time (dlopen of
  * libnccl.so.2, the one already in the process if any) and owns the communicator.  The reference uses NCCL

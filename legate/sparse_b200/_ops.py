@@ -417,6 +417,28 @@ def csr_scale(indptr, indices, data, d, mode: str, shape):
     return out
 
 
+def sddmm(indptr, indices, data, C, Dt, out=None):
+    """out[p] = data[p] * dot(C[i], Dt[j]) for every stored entry p = (i, j) through b2s_sddmm_csr (replaces task
+    CSR_SDDMM, sparse/csr.py:1243-1314).  C is (nrows, k), Dt is D transposed, (ncols, k); rows of either may be strided,
+    the k entries of a row must be contiguous.  `out` (data's shape and dtype) may be preallocated, e.g. for graph
+    capture; the launch neither syncs nor allocates."""
+    _chk_dev(indptr, indices, data, C, Dt, out)
+    nrows, k = C.shape
+    ncols = Dt.shape[0]
+    assert C.dtype == Dt.dtype == data.dtype and C.ndim == 2 and Dt.ndim == 2 and Dt.shape[1] == k
+    assert indptr.shape[0] == nrows + 1
+    assert k <= 1 or ((nrows == 0 or C.stride(1) == 1) and (ncols == 0 or Dt.stride(1) == 1))
+    ldc = C.stride(0) if nrows > 1 else max(k, 1)
+    ldd = Dt.stride(0) if ncols > 1 else max(k, 1)
+    if out is None:
+        out = torch.empty(data.shape, dtype=data.dtype, device=data.device)
+    assert out.dtype == data.dtype and out.shape == data.shape and out.is_contiguous()
+    _lib.check(L.b2s_sddmm_csr(vt_code(data.dtype), idx_code(indices.dtype), idx_code(indptr.dtype), nrows, ncols,
+                               int(data.shape[0]), k, ptr(indptr), ptr(indices.contiguous()), ptr(data.contiguous()),
+                               ptr(C), ldc, ptr(Dt), ldd, ptr(out), _stream()), "b2s_sddmm_csr")
+    return out
+
+
 def spgemm_row_work(a_indptr, a_indices, b_indptr) -> torch.Tensor:
     """Products per row of A @ B (int64 device tensor of len m): the chunk planner's measure of work / output size."""
     _chk_dev(a_indptr, a_indices, b_indptr)

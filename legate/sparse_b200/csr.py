@@ -741,6 +741,35 @@ class csr_array:
         data = _ops.csr_scale(A._indptr, A._indices, A._data, Dd, mode, self.shape)
         return csr_array._from_parts(A._indptr, A._indices, data, self.shape)
 
+    def sddmm(self, C, D):
+        """Sampled dense-dense product (reference csr.py:688-705): a new csr_array with A's structure (it shares A's
+        indptr and indices) whose value at each stored entry (i, j) is A[i, j] * (C @ D)[i, j], for C (m, k) and D (k, n)
+        given as numpy arrays or torch tensors.  Every stored entry is computed on its own: repeated columns, unsorted
+        rows and explicit zeros are kept, and k = 0 gives A.data * 0.  The dtype is np.result_type(A, C, D).
+
+        The kernel reads D transposed, an (n, k) array with contiguous rows.  When D.T already has unit inner stride
+        (D = K.T for a row-major (n, k) K, or a Fortran-ordered D) it is used as it is; otherwise D is copied once into
+        that layout, which costs a read and a write of n * k values (comparable to the product itself when k is large
+        and A has few entries per column).  C is copied only when its rows are not unit-stride."""
+        Cx = C if isinstance(C, (np.ndarray, torch.Tensor)) else np.asarray(C)
+        Dx = D if isinstance(D, (np.ndarray, torch.Tensor)) else np.asarray(D)
+        if Cx.ndim != 2 or Dx.ndim != 2:
+            raise ValueError(f"sddmm needs 2-D dense operands, got {Cx.ndim}-D and {Dx.ndim}-D")
+        m, n = self.shape
+        if Cx.shape[0] != m or Dx.shape[1] != n or Cx.shape[1] != Dx.shape[0]:
+            raise ValueError(f"inconsistent shapes {self.shape}, {tuple(Cx.shape)} and {tuple(Dx.shape)} for sddmm")
+        common = np.result_type(self.dtype, numpy_dtype(Cx.dtype), numpy_dtype(Dx.dtype))
+        if common.kind == "c":
+            raise NotImplementedError("complex sddmm is not implemented")
+        if common not in SUPPORTED_VALUE_DTYPES:
+            raise NotImplementedError(f"sddmm for dtype {common} is not implemented (float32/float64 kernels only)")
+        runtime.require_cuda("csr_array.sddmm")
+        A = self._promoted(common)
+        Cd = _dense_rows(Cx, common)
+        Dt = _dense_rows(Dx.T, common)
+        out = _ops.sddmm(A._indptr, A._indices, A._data, Cd, Dt)
+        return csr_array._from_parts(A._indptr, A._indices, out, self.shape)
+
     def eliminate_zeros(self):
         """Remove the explicitly stored zeros (either sign), in place."""
         keep = self._data != 0
@@ -807,6 +836,18 @@ def spgemm_csr_csr_csr(A: csr_array, B: csr_array) -> csr_array:
     C = csr_array._from_parts(c_ptr, c_idx, c_val, (A.shape[0], B.shape[1]))
     C.spgemm_info = info
     return C
+
+
+def _dense_rows(a, dtype):
+    """A 2-D operand as a device tensor of `dtype` whose rows are unit-stride and do not overlap (the row stride may be
+    larger than a row): a tensor already in that form is used without a copy."""
+    if not isinstance(a, torch.Tensor):
+        return to_device(a, dtype=dtype)   # numpy: C-ordered (a view when it already is) and copied to the device
+    t = a.to(device=runtime.device, dtype=torch_dtype(dtype))
+    rows, k = t.shape
+    if (k > 1 and t.stride(1) != 1) or (rows > 1 and t.stride(0) < k):
+        t = t.contiguous()
+    return t
 
 
 def _as_sparse_operand(other):

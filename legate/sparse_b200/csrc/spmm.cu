@@ -38,29 +38,6 @@ namespace b2s {
 
 constexpr int SPMM_THREADS = 256;
 
-template <typename V, int VEC> struct Pack;
-template <typename V> struct Pack<V, 1> {
-  V v[1];
-  __device__ __forceinline__ void load(const V* p) { v[0] = __ldg(p); }
-  __device__ __forceinline__ void store(V* p) const { p[0] = v[0]; }
-};
-template <> struct Pack<float, 4> {
-  float v[4];
-  __device__ __forceinline__ void load(const float* p) {
-    float4 t = __ldg(reinterpret_cast<const float4*>(p));
-    v[0] = t.x; v[1] = t.y; v[2] = t.z; v[3] = t.w;
-  }
-  __device__ __forceinline__ void store(float* p) const { *reinterpret_cast<float4*>(p) = make_float4(v[0], v[1], v[2], v[3]); }
-};
-template <> struct Pack<double, 2> {
-  double v[2];
-  __device__ __forceinline__ void load(const double* p) {
-    double2 t = __ldg(reinterpret_cast<const double2*>(p));
-    v[0] = t.x; v[1] = t.y;
-  }
-  __device__ __forceinline__ void store(double* p) const { *reinterpret_cast<double2*>(p) = make_double2(v[0], v[1]); }
-};
-
 template <typename V, typename I, typename P, int VEC, int CH>
 __global__ void __launch_bounds__(SPMM_THREADS)
 spmm_row_kernel(int64_t nrows, int64_t k, const P* __restrict__ indptr, const I* __restrict__ indices,
