@@ -386,6 +386,17 @@ int         b2s_sddmm_csr(int vt, int it, int pt, int64_t nrows, int64_t ncols, 
                           const void* indptr, const void* indices, const void* vals,
                           const void* C, int64_t ldc, const void* Dt, int64_t ldd, void* out, void* stream);
 
+/* ---- tropical SpMV: y[i, :] = lexicographic max of the zero vector and x[j, :] over every stored entry (i, j) ----
+ * Replaces CSRTropicalSpMV::gpu_variant (src/sparse/array/csr/tropical_spmv.cu:26-56) and tropical_spmv
+ * (sparse/csr.py:365-424).  x is (ncols x nfields) and y (nrows x nfields), both int64 and row-major with row strides
+ * ldx, ldy >= nfields; fields compare as signed int64, field 0 the most significant.  A's values are not read: every
+ * stored entry (explicit zeros, repeated columns) is an edge.  An empty row, or one whose neighbours are all
+ * lexicographically negative, gives zeros.  The result is exact and does not depend on the index widths.  x and y must
+ * not overlap.  No host sync, no allocation: capturable in a CUDA graph. */
+int         b2s_tropical_spmv_csr(int it, int pt, int64_t nrows, int64_t ncols, int64_t nnz, int64_t nfields,
+                                  const void* indptr, const void* indices, const void* x, int64_t ldx,
+                                  void* y, int64_t ldy, void* stream);
+
 /* ---- multi-GPU: NCCL communicator owned by the library (SURVEY 8b) -----------------------------------------
  * For hosts without torch.distributed (and for multi-node runs): the library binds NCCL at run time (dlopen of
  * libnccl.so.2, the one already in the process if any) and owns the communicator.  The reference uses NCCL

@@ -439,6 +439,26 @@ def sddmm(indptr, indices, data, C, Dt, out=None):
     return out
 
 
+def tropical_spmv(indptr, indices, x, y=None):
+    """y[i] = lexicographic max of 0 and x[j] over the stored entries (i, j) through b2s_tropical_spmv_csr (replaces
+    task CSR_SPMV_ROW_SPLIT_TROPICAL_SEMIRING, sparse/csr.py:365-424).  x is (ncols, F) int64 and y (nrows, F) int64;
+    rows of either may be strided, the F fields of a row must be contiguous, and y must not overlap x.  `y` may be
+    preallocated, e.g. for graph capture; the launch neither syncs nor allocates."""
+    _chk_dev(indptr, indices, x, y)
+    nrows = indptr.shape[0] - 1
+    ncols, nf = x.shape
+    assert x.dtype == torch.int64 and (nf <= 1 or ncols == 0 or x.stride(1) == 1)
+    if y is None:
+        y = torch.empty((nrows, nf), dtype=torch.int64, device=x.device)
+    assert y.dtype == torch.int64 and tuple(y.shape) == (nrows, nf) and (nf <= 1 or nrows == 0 or y.stride(1) == 1)
+    ldx = x.stride(0) if ncols > 1 else max(nf, 1)
+    ldy = y.stride(0) if nrows > 1 else max(nf, 1)
+    _lib.check(L.b2s_tropical_spmv_csr(idx_code(indices.dtype), idx_code(indptr.dtype), nrows, ncols,
+                                       int(indices.shape[0]), nf, ptr(indptr), ptr(indices.contiguous()), ptr(x), ldx,
+                                       ptr(y), ldy, _stream()), "b2s_tropical_spmv_csr")
+    return y
+
+
 def spgemm_row_work(a_indptr, a_indices, b_indptr) -> torch.Tensor:
     """Products per row of A @ B (int64 device tensor of len m): the chunk planner's measure of work / output size."""
     _chk_dev(a_indptr, a_indices, b_indptr)

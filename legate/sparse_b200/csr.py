@@ -770,6 +770,50 @@ class csr_array:
         out = _ops.sddmm(A._indptr, A._indices, A._data, Cd, Dt)
         return csr_array._from_parts(A._indptr, A._indices, out, self.shape)
 
+    def tropical_spmv(self, other, out=None):
+        """Lexicographic-max product (reference csr.py:365-424, kernel tropical_spmv.cu:26-56): for x of shape (n, F),
+        row i of the (m, F) int64 result is the lexicographic maximum of the zero vector and of x[j, :] over every
+        stored entry (i, j).  Fields compare as signed int64, field 0 the most significant.  Only A's structure counts:
+        its values and dtype are ignored, and explicit zeros and repeated columns are edges like any other.  An empty
+        row, or one whose neighbours are all lexicographically negative, gives zeros.  The result is exact.
+
+        x must be 2-D with n rows (else ValueError).  The reference leaves dtype checks open; here any integer dtype is
+        accepted and cast to int64 (uint64 values above 2^63 - 1 wrap), and float, complex and bool raise TypeError.
+        The result has x's array kind, as in `dot`: a numpy x gives numpy, a torch CUDA x a torch CUDA tensor, used
+        without a copy when it is int64 with unit-stride rows.  `out` may be a numpy array or a torch tensor of shape
+        (m, F) and dtype int64 (else ValueError), and must not overlap x (ValueError): the kernel reads x rows while
+        other rows of the result are written.  Every argument is checked before a device is touched."""
+        x = other if isinstance(other, (np.ndarray, torch.Tensor)) else np.asarray(other)
+        if x.ndim != 2:
+            raise ValueError(f"tropical_spmv needs a 2-D operand, got {x.ndim}-D")
+        m, n = self.shape
+        if x.shape[0] != n:
+            raise ValueError(f"inconsistent shapes {self.shape} and {tuple(x.shape)} for tropical_spmv")
+        if not _is_integer_dtype(x.dtype):
+            raise TypeError(f"tropical_spmv needs an integer operand, got {x.dtype}")
+        nf = int(x.shape[1])
+        if out is not None:
+            int64_out = ((isinstance(out, np.ndarray) and out.dtype == np.int64)
+                         or (isinstance(out, torch.Tensor) and out.dtype == torch.int64))
+            if not int64_out or tuple(out.shape) != (m, nf):
+                raise ValueError(f"out must be an int64 numpy array or torch tensor of shape {(m, nf)}")
+            if _overlaps(out, x):
+                raise ValueError("out overlaps the operand of tropical_spmv")
+        runtime.require_cuda("csr_array.tropical_spmv")
+        on_device = is_device_array(x) and x.is_cuda
+        xd = _dense_rows(x, np.int64)
+        direct = (isinstance(out, torch.Tensor) and out.is_cuda and (nf <= 1 or m == 0 or out.stride(1) == 1)
+                  and (m <= 1 or out.stride(0) >= nf))
+        y = _ops.tropical_spmv(self._indptr, self._indices, xd, out if direct else None)
+        if out is None:
+            return y if on_device else to_host(y)
+        if not direct:
+            if isinstance(out, torch.Tensor):
+                out.copy_(y)
+            else:
+                out[...] = to_host(y)
+        return out
+
     def eliminate_zeros(self):
         """Remove the explicitly stored zeros (either sign), in place."""
         keep = self._data != 0
@@ -848,6 +892,30 @@ def _dense_rows(a, dtype):
     if (k > 1 and t.stride(1) != 1) or (rows > 1 and t.stride(0) < k):
         t = t.contiguous()
     return t
+
+
+def _is_integer_dtype(dt) -> bool:
+    if isinstance(dt, torch.dtype):
+        return not (dt.is_floating_point or dt.is_complex or dt == torch.bool)
+    return np.dtype(dt).kind in "iu"
+
+
+def _overlaps(a, b) -> bool:
+    """True when the memory ranges of two arrays intersect: numpy arrays and CPU tensors in host memory, or tensors on
+    one device."""
+    def span(t):
+        if isinstance(t, np.ndarray):
+            if t.size == 0:
+                return None
+            lo, hi = np.lib.array_utils.byte_bounds(t)
+            return "cpu", lo, hi
+        if t.numel() == 0:
+            return None
+        lo = t.data_ptr()
+        return str(t.device), lo, lo + (sum((s - 1) * st for s, st in zip(t.shape, t.stride())) + 1) * t.element_size()
+
+    sa, sb = span(a), span(b)
+    return sa is not None and sb is not None and sa[0] == sb[0] and sa[1] < sb[2] and sb[1] < sa[2]
 
 
 def _as_sparse_operand(other):
