@@ -96,13 +96,12 @@ class coo_array:
         """Assembly on the GPU by the library's own kernels (b2s_coo_to_csr, csrc/convert.cu): counting sort of the
         triplets by row, scan of the row counts (nnz_to_pos, reference base.py:30-48), per-row bitonic sort by column.
         Real float32/float64 values; other dtypes (complex) take the tensor-op route below."""
-        from .csr import _INT32_MAX, _force_wide, csr_array
+        from .csr import _index_dtype, _indptr_dtype, csr_array
 
         vals, rows, cols = self._dev
         m, n = self.shape
-        wide = _force_wide()
-        ptr_dt = torch.int64 if (wide or vals.shape[0] > _INT32_MAX) else torch.int32
-        idx_dt = torch.int64 if (wide or max(m, n) > _INT32_MAX) else torch.int32
+        ptr_dt = _indptr_dtype(vals.shape[0])
+        idx_dt = _index_dtype(max(m, n))
         if vals.dtype in (torch.float32, torch.float64) and vals.is_cuda:
             from . import _ops
 

@@ -41,6 +41,23 @@ def _force_wide() -> bool:
     return os.environ.get("B2S_INDEX_WIDTH", "") == "64"
 
 
+def _indptr_dtype(nnz: int) -> torch.dtype:
+    """Row-pointer dtype of a CSR matrix with `nnz` stored entries: int32 only below 2^31 - 1 entries, the bound the
+    kernels' entry points accept an int32 indptr for."""
+    return torch.int32 if nnz < _INT32_MAX and not _force_wide() else torch.int64
+
+
+def _index_dtype(largest: int) -> torch.dtype:
+    """Column-index dtype for indices up to `largest`."""
+    return torch.int32 if largest <= _INT32_MAX and not _force_wide() else torch.int64
+
+
+def _entry_rows(indptr: torch.Tensor) -> torch.Tensor:
+    """The int64 row of every stored entry of a CSR matrix with row pointers `indptr`."""
+    ptr = indptr.to(torch.int64)
+    return torch.repeat_interleave(ptr[1:] - ptr[:-1])
+
+
 def cast_to_common_type(*args):
     """numpy.result_type promotion of the operands (reference sparse/utils.py:134-140)."""
     dts = [numpy_dtype(a.dtype) for a in args]
@@ -58,8 +75,7 @@ class csr_array:
     def __init__(self, arg, shape=None, dtype=None, copy=False):
         from .module import is_sparse_matrix
 
-        self._plan = None
-        self._plan_key = None
+        self._cache = {}
         if isinstance(arg, torch.Tensor) and arg.ndim == 2:
             arg = to_host(arg)
         if isinstance(arg, np.ndarray):
@@ -117,18 +133,10 @@ class csr_array:
 
     # -- storage ------------------------------------------------------------------------------------
     def _set_arrays(self, indptr, indices, data, copy=False):
-        nnz = int(data.shape[0])
-        wide = _force_wide()
-        ptr_dt = np.int64 if (wide or nnz > _INT32_MAX) else np.int32
-        self._indptr = to_device(indptr, dtype=ptr_dt, copy=copy)
-        if isinstance(indices, torch.Tensor):
-            idx_dt = np.int64 if wide else np.int32
-            if not wide and indices.numel() and int(indices.max()) > _INT32_MAX:
-                idx_dt = np.int64
-        else:
+        self._indptr = to_device(indptr, dtype=_indptr_dtype(int(data.shape[0])), copy=copy)
+        if not isinstance(indices, torch.Tensor):
             indices = np.asarray(indices)
-            idx_dt = np.int64 if (wide or (indices.size and int(indices.max()) > _INT32_MAX)) else np.int32
-        self._indices = to_device(indices, dtype=idx_dt, copy=copy)
+        self._indices = to_device(indices, dtype=_index_dtype(int(indices.max()) if len(indices) else 0), copy=copy)
         self._data = to_device(data, copy=copy)
 
     # reference exposes `.data` / `.indices` as device arrays (csr.py:264-287); `.indptr` is added
@@ -141,10 +149,7 @@ class csr_array:
     def data(self, value):
         self._data = to_device(value)
         self.dtype = numpy_dtype(self._data.dtype)
-        # derived matrices (promoted copy, real expansion of complex values, transpose) follow the values
-        self.__dict__.pop("_promo_cache", None)
-        self.__dict__.pop("_expansion", None)
-        self.__dict__.pop("_transposed", None)
+        self._cache.clear()
 
     @property
     def indices(self):
@@ -153,7 +158,7 @@ class csr_array:
     @indices.setter
     def indices(self, value):
         self._indices = to_device(value)
-        self._plan = None
+        self._cache.clear()
 
     @property
     def indptr(self):
@@ -170,8 +175,7 @@ class csr_array:
     @classmethod
     def _from_parts(cls, indptr, indices, data, shape):
         obj = cls.__new__(cls)
-        obj._plan = None
-        obj._plan_key = None
+        obj._cache = {}
         obj._indptr, obj._indices, obj._data = indptr, indices, data
         obj.shape = tuple(int(i) for i in shape)
         obj.dtype = numpy_dtype(data.dtype)
@@ -211,10 +215,7 @@ class csr_array:
     def tocoo(self, copy=False):
         from .coo import coo_array
 
-        counts = (self._indptr[1:] - self._indptr[:-1]).to(torch.int64)
-        rows = torch.repeat_interleave(
-            torch.arange(self.shape[0], dtype=torch.int64, device=self.device), counts
-        )
+        rows = _entry_rows(self._indptr)
         return coo_array((self._data.clone() if copy else self._data, (rows, self._indices)), shape=self.shape)
 
     def to_scipy_sparse_csr(self):
@@ -243,16 +244,14 @@ class csr_array:
             # the library's own kernels (b2s_csr_transpose, csrc/convert.cu): counting sort by column + per-row sort
             t_ptr, t_idx, t_val = _ops.csr_transpose(self._indptr, self._indices, self._data, self.shape)
             return csr_array._from_parts(t_ptr, t_idx, t_val, (ncols, nrows))
-        counts = (self._indptr[1:] - self._indptr[:-1]).to(torch.int64)
-        rows = torch.repeat_interleave(torch.arange(nrows, dtype=torch.int64, device=dev), counts)
+        rows = _entry_rows(self._indptr)
         cols = self._indices.to(torch.int64)
         order = torch.argsort(cols * max(nrows, 1) + rows)
         t_counts = torch.bincount(cols, minlength=ncols)
         t_indptr = torch.zeros(ncols + 1, dtype=torch.int64, device=dev)
         torch.cumsum(t_counts, 0, out=t_indptr[1:])
-        idx_dt = torch.int64 if (_force_wide() or nrows > _INT32_MAX) else torch.int32
-        ptr_dt = torch.int64 if (_force_wide() or self.nnz > _INT32_MAX) else torch.int32
-        return csr_array._from_parts(t_indptr.to(ptr_dt), rows[order].to(idx_dt), self._data[order], (ncols, nrows))
+        return csr_array._from_parts(t_indptr.to(_indptr_dtype(self.nnz)), rows[order].to(_index_dtype(nrows)),
+                                     self._data[order], (ncols, nrows))
 
     T = property(transpose)
 
@@ -266,29 +265,44 @@ class csr_array:
             return d[: min(rows, cols)]
         return to_device(self.to_scipy_sparse_csr().diagonal())
 
+    # -- what is derived from the arrays, cached -------------------------------------------------------
+    def _stamp(self):
+        """Pointer and version counter of indptr, indices and data.  An in-place edit of any of them changes it;
+        assigning a new array does not always (a new tensor may reuse a freed one's address and version), so every
+        assignment clears `_cache` as well."""
+        p, i, d = self._indptr, self._indices, self._data
+        return p.data_ptr(), p._version, i.data_ptr(), i._version, d.data_ptr(), d._version
+
+    def _derived(self, kind, extra, build):
+        """The derivative `kind` of the arrays (SpMV plan, promoted copy, transpose, ...) for the parameters `extra`:
+        `build()` runs again whenever the stamp or `extra` differs from the cached one.  One slot per kind, so a caller
+        switching parameters on one matrix does not pile up device buffers."""
+        stamp = self._stamp()
+        hit = self._cache.get(kind)
+        if hit is None or hit[0] != stamp or hit[1] != extra:
+            hit = self._cache[kind] = (stamp, extra, build())
+        return hit[2]
+
     # -- the hot path -----------------------------------------------------------------------------------
     def _get_plan(self, tma_only: bool = False):
         """Tile plan for the SpMV kernel, built once per structure and cached (the reference caches
         its image partitions per store the same way, sparse/partition.py:96-120).  `tma_only`: the plan must
-        launch the TMA tile kernel (accumulating / exchange-fused products); sticky once requested."""
+        launch the TMA tile kernel (accumulating / exchange-fused products); sticky once requested.  A packed plan
+        holds its own copy of the structure, and a coded one of the values, so an in-place edit builds a new plan --
+        a new one, never a rewrite of the old pack buffer, which a captured graph may still read."""
         from . import _lib
 
         tma_only = bool(tma_only or getattr(self, "_plan_tma_only", False))
         self._plan_tma_only = tma_only
-        # the versions: a packed plan holds its own copy of the structure, and a coded one of the values, so an
-        # in-place edit of indices / indptr / data (same pointers) must build a new plan -- a new one, never a rewrite
-        # of the old pack buffer, which a captured graph may still read
-        key = (self._indptr.data_ptr(), self._indptr._version, self._indices.data_ptr(), self._indices._version,
-               self._data.data_ptr(), self._data._version,
-               int(_lib.lib.b2s_spmv_get_config()), self.dtype.itemsize, self.nnz, tma_only)
-        if self._plan is None or self._plan_key != key:
+
+        def build():
             plan = _ops.spmv_plan(self._indptr, self._indices, self.shape, self.nnz, self.dtype, tma_only=tma_only)
             if self._data.is_contiguous():
                 plan = _ops.spmv_plan_code(plan, self._indptr, self._indices, self._data)
                 plan = _ops.spmv_plan_templates(plan, self._indptr, self._indices, self._data)
-            self._plan = plan
-            self._plan_key = key
-        return self._plan
+            return plan
+
+        return self._derived("plan", (int(_lib.lib.b2s_spmv_get_config()), tma_only), build)
 
     # -- column-split SpMV (reference csr.py:869-927 / spmv.cu:125-153: x partitioned, y reduced) -------------------
     @staticmethod
@@ -308,30 +322,13 @@ class csr_array:
             scattered = bool(getattr(self._get_plan(), "scattered", False))
             nblocks = max(2, min(16, -(-n * self.dtype.itemsize // self._col_block_bytes()))) if scattered else 2
         nblocks = max(1, min(int(nblocks), max(n, 1)))
-        key = (self._indptr.data_ptr(), self._indices.data_ptr(), self._data.data_ptr(), self._data._version, self.nnz,
-               nblocks)
-        hit = self.__dict__.get("_colsplit")
-        if hit is not None and hit[0] == key:
-            return hit[1]
-        T = -(-n // nblocks)
-        idx = self._indices
-        nrows = self.shape[0]
-        counts = (self._indptr[1:] - self._indptr[:-1]).to(torch.int64)
-        rows = torch.repeat_interleave(torch.arange(nrows, device=idx.device, dtype=torch.int64), counts)
-        blocks = []
-        for q in range(nblocks):
-            mask = (idx >= q * T) & (idx < min((q + 1) * T, n))
-            nnz_q = int(mask.sum())
-            if nnz_q == 0:
-                continue
-            cnt = torch.bincount(rows[mask], minlength=nrows)
-            ip = torch.zeros(nrows + 1, dtype=torch.int64, device=idx.device)
-            torch.cumsum(cnt, 0, out=ip[1:])
-            B = csr_array._from_parts(ip.to(self._indptr.dtype), idx[mask].contiguous(), self._data[mask].contiguous(),
-                                      self.shape)
-            blocks.append((B, B._get_plan(tma_only=True)))
-        self.__dict__["_colsplit"] = (key, blocks)
-        return blocks
+
+        def build():
+            T = -(-n // nblocks)
+            blocks = _column_blocks(self, [(q * T, min((q + 1) * T, n)) for q in range(nblocks)])
+            return [(B, B._get_plan(tma_only=True)) for B in blocks if B is not None]
+
+        return self._derived("colsplit", nblocks, build)
 
     def _dot_col_split(self, xd, y, nblocks=None):
         """y = A @ xd as a sum over column blocks: the first block writes y, the others accumulate (b2s_spmv_csr_add)."""
@@ -360,7 +357,7 @@ class csr_array:
         nblocks = -(-xbytes // self._col_block_bytes())
         if self.nnz < 4 * nblocks * max(self.shape[0], 1):
             return False
-        if "_colsplit" in self.__dict__:
+        if "colsplit" in self._cache:
             return True
         # the blocks are a second copy of the matrix (+ one indptr per block, + transient masks while they are cut):
         # only when that fits comfortably in what the device has free
@@ -376,12 +373,7 @@ class csr_array:
         so a mixed-dtype SpMV does not re-cast the matrix on every call."""
         if self.dtype == common:
             return self
-        cache = self.__dict__.setdefault("_promo_cache", {})
-        hit = cache.get(common)
-        stamp = (self._data.data_ptr(), self._data._version)   # in-place edits of .data keep the pointer
-        if hit is None or hit[0] != stamp:
-            cache[common] = (stamp, self.astype(common, copy=False))
-        return cache[common][1]
+        return self._derived(("promoted", common), None, lambda: self.astype(common, copy=False))
 
     def _dot_host_pipelined(self, x: np.ndarray, out, plan):
         """y = A @ x for HOST vectors, software-pipelined over the plan's row chunks.
@@ -410,17 +402,16 @@ class csr_array:
         complex entry a at (r, c) becomes the block [[re a, -im a], [im a, re a]] at rows 2r, 2r+1 / columns
         2c, 2c+1.  Built once per matrix with tensor ops and cached, so a complex SpMV is ONE launch of the real
         SpMV kernel on interleaved (re, im) storage -- which is exactly how complex vectors sit in memory."""
-        hit = self.__dict__.get("_expansion")
-        key = (self._data.data_ptr(), self._data._version, self._indptr.data_ptr(), np.dtype(rdt))
-        if hit is not None and hit[0] == key:
-            return hit[1]
+        return self._derived("expansion", np.dtype(rdt), lambda: self._make_real_expansion(rdt))
+
+    def _make_real_expansion(self, rdt):
         m, n = self.shape
         dev = self.device
         nnz = self.nnz
         tdt = torch_dtype(rdt)
         ptr64 = self._indptr.to(torch.int64)
         lens = ptr64[1:] - ptr64[:-1]
-        rows = torch.repeat_interleave(torch.arange(m, dtype=torch.int64, device=dev), lens)
+        rows = _entry_rows(ptr64)
         q = torch.arange(nnz, dtype=torch.int64, device=dev) - ptr64[rows]      # position inside its row
         top = 4 * ptr64[rows] + 2 * q                                           # slot of (2r, 2c)
         bot = top + 2 * lens[rows]                                              # slot of (2r+1, 2c)
@@ -435,12 +426,8 @@ class csr_array:
         e_ptr[0:2 * m:2] = 4 * ptr64[:-1]
         e_ptr[1:2 * m:2] = 4 * ptr64[:-1] + 2 * lens
         e_ptr[2 * m] = 4 * nnz
-        wide = _force_wide()
-        idx_dt = torch.int64 if (wide or 2 * n > _INT32_MAX) else torch.int32
-        ptr_dt = torch.int64 if (wide or 4 * nnz > _INT32_MAX) else torch.int32
-        E = csr_array._from_parts(e_ptr.to(ptr_dt), e_idx.to(idx_dt), e_val, (2 * m, 2 * n))
-        self._expansion = (key, E)
-        return E
+        return csr_array._from_parts(e_ptr.to(_indptr_dtype(4 * nnz)), e_idx.to(_index_dtype(2 * n)), e_val,
+                                     (2 * m, 2 * n))
 
     def _dot_complex(self, other, out):
         """A @ x / A @ X when the resolved dtype is complex (the reference dispatches its SpMV / SpMM tasks over
@@ -628,10 +615,7 @@ class csr_array:
         if other.ndim != 2:
             raise NotImplementedError
         assert other.shape[1] == self.shape[0]
-        key = (self._indptr.data_ptr(), self._indices.data_ptr(), self._data.data_ptr(), self._data._version, self.nnz)
-        if getattr(self, "_transposed", None) is None or self._transposed[0] != key:
-            self._transposed = (key, self.transpose())
-        At = self._transposed[1]
+        At = self._derived("transpose", None, self.transpose)
         if isinstance(other, torch.Tensor):
             return At.dot(other.t().contiguous()).t().contiguous()
         return np.ascontiguousarray(At.dot(np.ascontiguousarray(other.T)).T)
@@ -647,13 +631,6 @@ class csr_array:
         return self * -1
 
     # -- elementwise arithmetic (reference csr.py:760-776 __add__ / add, 1033-1148 mult / mult_dense) ------------------
-    def _invalidate(self):
-        """Drop the SpMV plan and every matrix derived from the arrays (after an in-place change of the structure)."""
-        self._plan = None
-        self._plan_key = None
-        for k in ("_promo_cache", "_expansion", "_transposed", "_colsplit"):
-            self.__dict__.pop(k, None)
-
     def _binop(self, other, op: str, reverse: bool = False):
         """self op other (other op self when `reverse`) for a sparse `other`; None when `other` is not sparse."""
         B = _as_sparse_operand(other)
@@ -673,8 +650,7 @@ class csr_array:
             raise NotImplementedError("complex elementwise operations are not implemented")
         if isinstance(other, torch.Tensor):
             D = torch.zeros(self.shape, dtype=torch_dtype(common), device=other.device)
-            counts = (self._indptr[1:] - self._indptr[:-1]).to(torch.int64)
-            rows = torch.repeat_interleave(torch.arange(self.shape[0], dtype=torch.int64, device=self.device), counts)
+            rows = _entry_rows(self._indptr)
             D.index_put_((rows.to(other.device), self._indices.to(device=other.device, dtype=torch.int64)),
                          self._data.to(device=other.device, dtype=D.dtype), accumulate=True)
         else:
@@ -824,7 +800,7 @@ class csr_array:
         self._indptr = kept[self._indptr.to(torch.int64)].to(self._indptr.dtype)
         self._indices = self._indices[keep]
         self._data = self._data[keep]
-        self._invalidate()
+        self._cache.clear()
 
     @property
     def has_sorted_indices(self) -> bool:
@@ -843,7 +819,7 @@ class csr_array:
         if self.has_sorted_indices:
             return
         self._indices, self._data = _ops.csr_sort_rows(self._indptr, self._indices.clone(), self._data.clone())
-        self._invalidate()
+        self._cache.clear()
 
     def balance(self):
         """No-op on a single device; kept for API parity (reference base.py:198-282 re-tiles the rows by
@@ -875,11 +851,29 @@ def spgemm_csr_csr_csr(A: csr_array, B: csr_array) -> csr_array:
     if a_ptr.dtype != b_ptr.dtype:
         a_ptr, b_ptr = a_ptr.to(torch.int64), b_ptr.to(torch.int64)
     c_ptr, c_idx, c_val, info = _ops.spgemm(a_ptr, a_idx, A._data, b_ptr, b_idx, B._data, A.shape, B.shape)
-    if info["nnz"] <= _INT32_MAX and not _force_wide():
-        c_ptr = c_ptr.to(torch.int32)
-    C = csr_array._from_parts(c_ptr, c_idx, c_val, (A.shape[0], B.shape[1]))
+    C = csr_array._from_parts(c_ptr.to(_indptr_dtype(info["nnz"])), c_idx, c_val, (A.shape[0], B.shape[1]))
     C.spgemm_info = info
     return C
+
+
+def _column_blocks(A: csr_array, ranges) -> list:
+    """[block or None per (lo, hi) in `ranges`]: block q holds the entries of A whose column lies in [lo_q, hi_q), with
+    global column ids and A's shape kept, or is None when there are none."""
+    idx = A._indices
+    nrows = A.shape[0]
+    rows = _entry_rows(A._indptr)
+    blocks = []
+    for lo, hi in ranges:
+        mask = (idx >= lo) & (idx < hi)
+        nnz = int(mask.sum())
+        if nnz == 0:
+            blocks.append(None)
+            continue
+        ip = torch.zeros(nrows + 1, dtype=torch.int64, device=idx.device)
+        torch.cumsum(torch.bincount(rows[mask], minlength=nrows), 0, out=ip[1:])
+        blocks.append(csr_array._from_parts(ip.to(_indptr_dtype(nnz)), idx[mask].contiguous(),
+                                            A._data[mask].contiguous(), A.shape))
+    return blocks
 
 
 def _dense_rows(a, dtype):
@@ -950,14 +944,9 @@ def _csr_binop(A: csr_array, B: csr_array, op: str) -> csr_array:
             b_idx, b_val = _ops.csr_sort_rows(b_ptr, b_idx.clone(), b_val.clone())
         c_ptr, c_idx, c_val, info = _ops.csr_binop(op, a_ptr, a_idx, a_val, b_ptr, b_idx, b_val, A.shape)
         assert c_idx is not None, "row sort left a decreasing row"
-    wide = _force_wide()
-    if info["nnz"] <= _INT32_MAX and not wide:
-        c_ptr = c_ptr.to(torch.int32)
-    if wide:
-        c_idx = c_idx.to(torch.int64)
-    elif c_idx.dtype == torch.int64 and A.shape[1] - 1 <= _INT32_MAX:
-        c_idx = c_idx.to(torch.int32)
-    return csr_array._from_parts(c_ptr, c_idx, c_val, A.shape)
+    if c_idx.dtype == torch.int64 or _force_wide():     # an int32 result keeps its width
+        c_idx = c_idx.to(_index_dtype(A.shape[1] - 1))
+    return csr_array._from_parts(c_ptr.to(_indptr_dtype(info["nnz"])), c_idx, c_val, A.shape)
 
 
 def spgemm_chunked(A: csr_array, B: csr_array, max_products: int = 1 << 31, keep: bool = False, on_chunk=None):
@@ -1013,9 +1002,7 @@ def spgemm_chunked(A: csr_array, B: csr_array, max_products: int = 1 << 31, keep
         for P_ in parts:
             ptrs.append(P_._indptr[1:].to(torch.int64) + off)
             off += P_.nnz
-        indptr = torch.cat(ptrs)
-        if off <= _INT32_MAX and not _force_wide():
-            indptr = indptr.to(torch.int32)
+        indptr = torch.cat(ptrs).to(_indptr_dtype(off))
         C = csr_array._from_parts(indptr, torch.cat([P_._indices for P_ in parts]) if parts else A._indices[:0],
                                   torch.cat([P_._data for P_ in parts]) if parts else A._data[:0], (m, B.shape[1]))
     return C, stats

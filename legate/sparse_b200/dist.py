@@ -28,7 +28,7 @@ import torch
 import torch.distributed as dist
 
 from . import _ops
-from .csr import csr_array
+from .csr import _column_blocks, _indptr_dtype, csr_array
 from .runtime import numpy_dtype, runtime, to_device, to_host, torch_dtype
 
 
@@ -573,33 +573,17 @@ class dist_csr_array:
                                               ticket=pc.ticket, epoch_add=0, epoch_bump=0, error=pc.error_word,
                                               accumulate=True)
                 slice_bytes = (hi - lo) * item
-                info = {"mode": "blocks", "blocks": blocks, "blocks_of": (A._data.data_ptr(), A._data._version),
-                        "descs": descs, "sends": sends, "recv_peers": recv_peers,
+                info = {"mode": "blocks", "blocks": blocks, "descs": descs, "sends": sends, "recv_peers": recv_peers,
                         "pc": pc, "cps": 16 if slice_bytes >= (1 << 22) else (4 if slice_bytes >= (1 << 18) else 1),
                         "order": [(self.rank + d) % self.nranks for d in range(1, self.nranks)]}
         self._fused[key] = info
         return info
 
     def _column_blocks(self, A: csr_array):
-        """{q: CSR of the entries of A whose column is owned by rank q (global column ids kept), or None if empty}."""
-        out = {}
-        idx = A.indices
-        nrows = A.shape[0]
-        counts_all = (A.indptr[1:] - A.indptr[:-1]).to(torch.int64)
-        rows = torch.repeat_interleave(torch.arange(nrows, device=idx.device, dtype=torch.int64), counts_all)
-        for q in range(self.nranks):
-            qlo, qhi = self.col_plan.rows(q)
-            mask = (idx >= qlo) & (idx < qhi)
-            nnz_q = int(mask.sum())
-            if nnz_q == 0:
-                out[q] = None
-                continue
-            cnt = torch.bincount(rows[mask], minlength=nrows)
-            indptr = torch.zeros(nrows + 1, dtype=torch.int64, device=idx.device)
-            torch.cumsum(cnt, 0, out=indptr[1:])
-            ptr_dt = torch.int32 if nnz_q < 2**31 - 1 else torch.int64
-            out[q] = csr_array._from_parts(indptr.to(ptr_dt), idx[mask].contiguous(), A.data[mask].contiguous(), A.shape)
-        return out
+        """{q: CSR of the entries of A whose column is owned by rank q (global column ids kept), or None if empty}, cut
+        once per state of A's arrays and cached with A's other derivatives."""
+        ranges = tuple(self.col_plan.rows(q) for q in range(self.nranks))
+        return A._derived("rank_blocks", ranges, lambda: dict(enumerate(_column_blocks(A, ranges))))
 
     def _dot_fused(self, info, A, x_full, out, w=None, dot_out=None):
         # the plan is looked up per launch, not kept in `info`: a coded plan holds the values, so an in-place edit of
@@ -618,10 +602,9 @@ class dist_csr_array:
             else:
                 _ops.spmv(A.indptr, A.indices, A.data, xin, out, A.shape, plan=A._get_plan())
             return out
-        if info["blocks_of"] != (A._data.data_ptr(), A._data._version):
-            # the column blocks hold copies of the values: cut them again (same structure, so the same tiles)
-            info["blocks"] = self._column_blocks(A)
-            info["blocks_of"] = (A._data.data_ptr(), A._data._version)
+        # the column blocks hold copies of the values: after an edit of A.data they are cut again (same structure, so
+        # the same tiles the descriptors name)
+        info["blocks"] = self._column_blocks(A)
         cur = torch.cuda.current_stream()
         if getattr(self, "_comm_stream", None) is None:
             self._comm_stream = torch.cuda.Stream()
@@ -844,8 +827,7 @@ def gather_matrix(A: "dist_csr_array") -> csr_array:
     torch.cumsum(all_counts, 0, out=indptr[1:])
     indices = torch.cat(_allgather_varlen(loc.indices, A.group))
     data = torch.cat(_allgather_varlen(loc.data, A.group))
-    ptr_dt = torch.int32 if int(indptr[-1]) < 2**31 - 1 else torch.int64
-    return csr_array._from_parts(indptr.to(ptr_dt), indices, data, A.shape)
+    return csr_array._from_parts(indptr.to(_indptr_dtype(int(indptr[-1]))), indices, data, A.shape)
 
 
 def spgemm(A: "dist_csr_array", B: "dist_csr_array") -> "dist_csr_array":

@@ -9,13 +9,12 @@ from __future__ import annotations
 import numpy as np
 import torch
 
-from .csr import csr_array
+from .csr import _indptr_dtype, csr_array
 from .runtime import runtime, torch_dtype
 
 
 def _finish(indptr64, indices, data, shape, nnz):
-    ptr_dt = torch.int32 if nnz < 2**31 - 1 else torch.int64
-    return csr_array._from_parts(indptr64.to(ptr_dt), indices, data, shape)
+    return csr_array._from_parts(indptr64.to(_indptr_dtype(nnz)), indices, data, shape)
 
 
 def laplacian_5pt(n1: int, n2: int, dtype=np.float64, row_lo: int = 0, row_hi: int | None = None,

@@ -351,11 +351,12 @@ def _cg_fused_loop(Ad: csr_array, comm, b, x, tol, maxiter, callback, conv_test_
         graphs = [_try_capture(lambda k=k: generic_iteration(k)) for k in (3, 1, 2)]   # index = k % 3
         if any(g is None for g in graphs):
             graphs = None
-    # the graphs replay the launches of the plan current at capture, whose codes are the values of Ad.data at that
-    # point: an in-place edit of Ad.data (from the callback) sends the loop back to eager launches, which re-plan
-    data_stamp = (Ad._data.data_ptr(), Ad._data._version)
+    # the graphs replay the launches of the plan current at capture, which holds its own copy of the structure and
+    # codes the values of that point: an edit of Ad's arrays (from the callback) sends the loop back to eager launches,
+    # which re-plan
+    stamp = Ad._stamp()
     while iters < maxiter:
-        if graphs is not None and (Ad._data.data_ptr(), Ad._data._version) != data_stamp:
+        if graphs is not None and Ad._stamp() != stamp:
             graphs = None
         if graphs is not None:
             graphs[iters % 3].replay()

@@ -163,8 +163,8 @@ def to_device(a, dtype=None, copy: bool = False) -> torch.Tensor:
             copy = False
         return t.clone() if copy else t
     arr = np.asarray(a)
-    if dtype is not None and arr.dtype != np.dtype(dtype):
-        arr = arr.astype(dtype)
+    if dtype is not None and arr.dtype != numpy_dtype(dtype):
+        arr = arr.astype(numpy_dtype(dtype))
     arr = np.ascontiguousarray(arr)
     if not arr.flags.writeable:
         arr = arr.copy()

@@ -10,7 +10,7 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from legate.sparse_b200 import _lib, _ops, gallery  # noqa: E402
-from legate.sparse_b200.csr import csr_array  # noqa: E402
+from legate.sparse_b200.csr import _column_blocks  # noqa: E402
 
 
 def time_fn(fn, reps=20, warm=3):
@@ -28,18 +28,7 @@ def time_fn(fn, reps=20, warm=3):
 def blocks_of(A, P):
     n = A.shape[1]
     T = (n + P - 1) // P
-    idx = A.indices
-    nrows = A.shape[0]
-    counts = (A.indptr[1:] - A.indptr[:-1]).to(torch.int64)
-    rows = torch.repeat_interleave(torch.arange(nrows, device=idx.device, dtype=torch.int64), counts)
-    out = []
-    for q in range(P):
-        mask = (idx >= q * T) & (idx < min((q + 1) * T, n))
-        cnt = torch.bincount(rows[mask], minlength=nrows)
-        ip = torch.zeros(nrows + 1, dtype=torch.int64, device=idx.device)
-        torch.cumsum(cnt, 0, out=ip[1:])
-        out.append(csr_array._from_parts(ip.to(torch.int32), idx[mask].contiguous(), A.data[mask].contiguous(), A.shape))
-    return out
+    return _column_blocks(A, [(q * T, min((q + 1) * T, n)) for q in range(P)])
 
 
 def l2_gran(set_bytes=0):
@@ -105,8 +94,7 @@ def main():
             for flavor in flavors:
                 tot, names = 0.0, set()
                 for B in blocks:
-                    B._plan = None
-                    pl = B._get_plan(tma_only=True)
+                    pl = B._get_plan(tma_only=True)     # a new config builds a new plan
                     if flavor is not None:
                         pl.set_flavor(flavor)
                     names.add(pl.kernel_name)
