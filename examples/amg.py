@@ -5,10 +5,15 @@ of the reference's examples/amg.py (a V-cycle as the preconditioner M of linalg.
 The matrix is diffusion2D(N, epsilon=0.1, theta=pi/4): the 9-point finite-difference stencil of the reference, built
 with `diags` from 9 offsets, with the stencil entries that cross the grid boundary dropped as the reference's
 stencil_grid drops them.  Per level, as in the reference:
-  * strength of connection with theta = 0 (the reference default): the matrix itself;
+  * strength of connection: with theta = 0 (the reference default, `--theta 0`) the matrix itself; with theta > 0 the
+    reference's filter: B = |A|, drop the entries with B_ij < theta * sqrt(B_ii * B_jj), then scale every entry by the
+    largest of its column, B.max(axis=0) (the column reduction of csr_array; scipy's sparse column maximum, densified,
+    with `--package scipy`);
   * aggregation by a distance-2 maximal independent set, MIS(2), found by repeated lexicographic-max products
     `C.tropical_spmv(x, out=z)` over (state, random priority, node id) triples, then one aggregate per MIS node
     (mis_aggregate);
+  * when a level's aggregation would keep more than 90% of its unknowns, coarsening has stalled and that level is the
+    coarsest (it only happens with theta > 0, once the coarse operators are dense);
   * the tentative prolongator T from fit_candidates (column sums by bincount), the smoothed prolongator
     P = T - (omega / rho) D^-1 A T with rho the spectral radius of D^-1 A by power iteration, R = P^T and
     A_c = R A P (two SpGEMMs), down to at most `max_coarse` unknowns, where a dense solve finishes the cycle.
@@ -20,7 +25,7 @@ neighbours are all lexicographically negative, gives zeros.  The reference's sci
 over the neighbours and omits that floor.  Every random value (MIS priorities, power-iteration start vectors) comes from
 one seeded numpy generator on the host, so both packages build the same aggregates.
 
-    python examples/amg.py -nodes 512 [--package scipy]
+    python examples/amg.py -nodes 512 [--theta 0.25] [--package scipy]
 """
 import argparse
 
@@ -34,6 +39,7 @@ ap.add_argument("-m", "--maxiter", type=int, default=1000)
 ap.add_argument("-t", "--tol", type=float, default=1e-8, help="CG stops when |r| < tol * |b|")
 ap.add_argument("--max-coarse", type=int, default=10)
 ap.add_argument("--seed", type=int, default=123)
+ap.add_argument("--theta", type=float, default=0.0, help="strength-of-connection threshold (0 keeps every coupling)")
 ap.add_argument("--package", default="b200")
 args = ap.parse_args()
 
@@ -61,6 +67,12 @@ if on_device:
 
     def transpose(P):
         return P.T
+
+    def entry_rows(B):
+        return torch.repeat_interleave(torch.diff(B.indptr.long()))
+
+    def column_max(B):
+        return B.max(axis=0)
 else:
 
     def dev(a):
@@ -94,6 +106,12 @@ else:
 
     def transpose(P):
         return P.T.tocsr()
+
+    def entry_rows(B):
+        return np.repeat(np.arange(B.shape[0]), np.diff(B.indptr))
+
+    def column_max(B):
+        return B.max(axis=0).toarray().ravel()
 
 
 def count(mask):
@@ -133,8 +151,16 @@ def diffusion2d(N, epsilon=0.1, theta=np.pi / 4):
 def strength(A, theta=0.0):
     """Strength of connection; theta = 0 (the reference default) keeps every coupling.  A stored zero couples nothing,
     and scipy prunes the zeros its products cancel to while this library keeps them, so the graph leaves them out
-    (a no-op for a matrix without stored zeros)."""
-    assert theta == 0.0
+    (a no-op for a matrix without stored zeros).  theta > 0 follows the reference: |A| without its weak couplings,
+    B_ij < theta * sqrt(B_ii * B_jj) (stored zeros among them), each entry divided by its column's maximum."""
+    if theta > 0:
+        B = abs(A)
+        D = B.diagonal()
+        rows, cols = entry_rows(B), B.indices
+        B.data *= B.data >= theta * (D[rows] * D[cols]) ** 0.5
+        B.eliminate_zeros()
+        B.data /= column_max(B)[B.indices]
+        return B
     if count(A.data == 0) == 0:
         return A
     C = A.copy()
@@ -234,7 +260,12 @@ def build_hierarchy(A, max_coarse):
     while levels[-1].A.shape[0] > max_coarse:
         L = levels[-1]
         L.D = L.A.diagonal()
-        agg, n_coarse = mis_aggregate(strength(L.A))
+        agg, n_coarse = mis_aggregate(strength(L.A, args.theta))
+        if n_coarse > 0.9 * L.A.shape[0]:
+            # coarsening has stalled (theta > 0 can filter a dense coarse level down to isolated nodes): this level
+            # becomes the coarsest and is solved directly
+            L.D = None
+            break
         T, B_coarse = fit_candidates(agg, n_coarse, L.B)
         L.P, L.rho = smooth_prolongator(L.A, T, L.D)
         L.R = transpose(L.P)
@@ -257,7 +288,7 @@ b = xp.ones(N)
 timer.start()
 levels, solve = build_hierarchy(A, args.max_coarse)
 build_ms = timer.stop()
-print(f"AMG hierarchy: {len(levels)} levels")
+print(f"AMG hierarchy: {len(levels)} levels" + (f", strength of connection theta = {args.theta:g}" if args.theta else ""))
 print("  level   unknowns   nonzeros")
 for i, L in enumerate(levels):
     print(f"{i:>7d} {L.A.shape[0]:>10d} {L.A.nnz:>10d}")

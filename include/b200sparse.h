@@ -397,6 +397,32 @@ int         b2s_tropical_spmv_csr(int it, int pt, int64_t nrows, int64_t ncols, 
                                   const void* indptr, const void* indices, const void* x, int64_t ldx,
                                   void* y, int64_t ldy, void* stream);
 
+/* ---- row reductions: out[i] = reduction `op` over row i of a CSR matrix (nrows x ncols) -------------------------
+ * Replaces the reference's sum (sparse/base.py:72-129, `A @ ones` through its SpMV task) and adds what scipy's
+ * max / min / argmax / argmin / count_nonzero compute; column reductions run on the transpose.
+ *   SUM           reads indptr, vals; out type vt: the sum of the stored values (+0 for an empty row), accumulated
+ *                 in fp64 and rounded once.  Repeated columns and unsorted rows are fine.
+ *   MAX / MIN     reads indptr, vals; out type vt: the extreme of the stored values, and of 0 when the row has fewer
+ *                 than ncols entries and explicit_only == 0; NaN when a stored value is NaN; 0 for an empty row.
+ *   ARGMAX / MIN  reads indptr, indices, vals; out int64: the smallest column at which the dense row attains that
+ *                 extreme.  An implicit zero's column is the first missing one (the first k whose entry is not k);
+ *                 a NaN row gives its smallest NaN column; an empty row gives 0.  explicit_only: stored entries only.
+ *   COUNT_NONZERO reads indptr, vals; out int64: stored values != 0 (NaN counts).
+ * MAX, MIN and COUNT_NONZERO need rows without repeated columns, ARG* strictly ascending columns; a matrix that breaks
+ * this gets an unspecified result, never an out-of-bounds read (column ids are only compared, never dereferenced).
+ * A zero result may be +0 or -0.  Each row is reduced in an order fixed by its length alone: bitwise repeatable and
+ * independent of the index widths.  `indices` may be NULL except for ARG*; `out` must not overlap the inputs.
+ * No host sync, no allocation: capturable in a CUDA graph. */
+#define B2S_REDUCE_SUM           0
+#define B2S_REDUCE_MAX           1
+#define B2S_REDUCE_MIN           2
+#define B2S_REDUCE_ARGMAX        3
+#define B2S_REDUCE_ARGMIN        4
+#define B2S_REDUCE_COUNT_NONZERO 5
+int         b2s_csr_reduce_rows(int op, int vt, int it, int pt, int64_t nrows, int64_t ncols, int64_t nnz,
+                                const void* indptr, const void* indices, const void* vals, int explicit_only,
+                                void* out, void* stream);
+
 /* ---- multi-GPU: NCCL communicator owned by the library (SURVEY 8b) -----------------------------------------
  * For hosts without torch.distributed (and for multi-node runs): the library binds NCCL at run time (dlopen of
  * libnccl.so.2, the one already in the process if any) and owns the communicator.  The reference uses NCCL

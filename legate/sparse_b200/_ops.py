@@ -459,6 +459,31 @@ def tropical_spmv(indptr, indices, x, y=None):
     return y
 
 
+REDUCE_OPS = {"sum": 0, "max": 1, "min": 2, "argmax": 3, "argmin": 4, "count_nonzero": 5}   # B2S_REDUCE_*
+
+
+def csr_reduce_rows(op: str, indptr, indices, data, ncols: int, explicit: bool = False, out=None):
+    """out[i] = reduction `op` over row i through b2s_csr_reduce_rows (op: "sum", "max", "min", "argmax", "argmin",
+    "count_nonzero"; see include/b200sparse.h for the implicit-zero, NaN and input rules).  `out` is data's dtype for
+    sum / max / min and int64 otherwise; it may be preallocated, e.g. for graph capture: the launch neither syncs nor
+    allocates.  `indices` may be None except for argmax / argmin."""
+    _chk_dev(indptr, indices, data, out)
+    code = REDUCE_OPS[op]
+    nrows = indptr.shape[0] - 1
+    odt = data.dtype if op in ("sum", "max", "min") else torch.int64
+    if out is None:
+        out = torch.empty(nrows, dtype=odt, device=data.device)
+    assert out.dtype == odt and tuple(out.shape) == (nrows,) and out.is_contiguous()
+    assert indptr.is_contiguous()
+    it = idx_code(indices.dtype) if indices is not None else _lib.I32
+    _lib.check(L.b2s_csr_reduce_rows(code, vt_code(data.dtype), it, idx_code(indptr.dtype), nrows, int(ncols),
+                                     int(data.shape[0]), ptr(indptr),
+                                     ptr(indices.contiguous()) if indices is not None else None,
+                                     ptr(data.contiguous()), int(bool(explicit)), ptr(out), _stream()),
+               "b2s_csr_reduce_rows")
+    return out
+
+
 def spgemm_row_work(a_indptr, a_indices, b_indptr) -> torch.Tensor:
     """Products per row of A @ B (int64 device tensor of len m): the chunk planner's measure of work / output size."""
     _chk_dev(a_indptr, a_indices, b_indptr)

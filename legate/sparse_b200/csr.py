@@ -790,6 +790,182 @@ class csr_array:
                 out[...] = to_host(y)
         return out
 
+    # -- reductions (scipy csr_array sum / mean / max / min / argmax / argmin / count_nonzero; csrc/reduce.cu) ----------
+    def _canonical(self):
+        """(indptr, indices, data) of A with sorted rows and repeated columns summed -- what `A.toarray()` sees, explicit
+        zeros kept.  Built once per stamp from a sorted clone when a row is unsorted; the merge of repeated columns runs
+        the row-sum kernel over the runs of equal columns.  Without either, it is A's own arrays (no copy)."""
+        return self._derived("canonical", None, lambda: _canonical_parts(self, rows_sorted=False))
+
+    def _canonical_t(self):
+        """The canonical form of the cached transpose (the one `X @ A` uses): its rows, A's columns, are sorted already."""
+        At = self._derived("transpose", None, self.transpose)
+        return self._derived("canonical_t", None, lambda: _canonical_parts(At, rows_sorted=True))
+
+    def _check_reduction(self, axis, what):
+        """`axis` as None, 0 or 1, after the checks that need no device: ValueError for any other axis,
+        NotImplementedError for data other than float32 / float64."""
+        if axis is not None:
+            if isinstance(axis, (bool, np.bool_)) or not isinstance(axis, (int, np.integer)) or not -2 <= axis <= 1:
+                raise ValueError(f"axis {axis!r} out of range for a 2-D sparse array (None, 0, 1, -2 or -1)")
+            axis = int(axis) % 2
+        if self.dtype not in SUPPORTED_VALUE_DTYPES:
+            raise NotImplementedError(f"csr_array.{what} for dtype {self.dtype} is not implemented (float32/float64 only)")
+        return axis
+
+    def _reduce_axis(self, op, axis, explicit=False):
+        """1-D device tensor: `op` over every row (axis 1) or column (axis 0).  Sums read A (or its transpose) as it
+        is; the other reductions read the canonical form."""
+        m, n = self.shape
+        if self.nnz == 0:       # every row or column is empty: no transpose to build
+            ptr_ = torch.zeros(self.shape[1 - axis] + 1, dtype=torch.int32, device=self.device)
+            return _ops.csr_reduce_rows(op, ptr_, self._indices, self._data, n if axis == 1 else m, explicit)
+        if op == "sum":
+            B = self if axis == 1 else self._derived("transpose", None, self.transpose)
+            ptr_, idx, dat = B._indptr, B._indices, B._data
+        else:
+            ptr_, idx, dat = self._canonical() if axis == 1 else self._canonical_t()
+        return _ops.csr_reduce_rows(op, ptr_, idx if op in ("argmax", "argmin") else None, dat, n if axis == 1 else m,
+                                    explicit)
+
+    def sum(self, axis=None, dtype=None, out=None):
+        """Sum of all entries (axis None: a numpy scalar), of every column (axis 0: a length-n CUDA tensor) or of every
+        row (axis 1: length m).  Rows are summed by the kernel in fp64 in an order fixed by their length, then rounded
+        once to `dtype` (default: the data's); float32 data with dtype float64 is summed from a cached float64 copy.
+        axis None is the sum of the stored values (fp64, one sync).  `out`: a numpy array or torch tensor of the
+        result's shape and dtype.  A column reduction builds a transposed copy of A once and keeps it in A's cache (the
+        one `X @ A` uses) until A's arrays change."""
+        axis = self._check_reduction(axis, "sum")
+        rdt = self._reduction_dtype(dtype, "sum")
+        _check_reduction_out(out, () if axis is None else (self.shape[1 - axis],), rdt)
+        runtime.require_cuda("csr_array.sum")
+        A = self._promoted(rdt) if rdt.itemsize > self.dtype.itemsize else self
+        if axis is None:
+            return _deliver_scalar(rdt.type(float(A._data.sum(dtype=torch.float64))), out)
+        v = A._reduce_axis("sum", axis)
+        return _deliver_vector(v.to(torch_dtype(rdt)), out)
+
+    def mean(self, axis=None, dtype=None, out=None):
+        """`sum(axis, dtype)` divided by shape[axis] (by m * n for axis None); same result kinds and `out` as sum."""
+        axis = self._check_reduction(axis, "mean")
+        rdt = self._reduction_dtype(dtype, "mean")
+        _check_reduction_out(out, () if axis is None else (self.shape[1 - axis],), rdt)
+        count = self.shape[0] * self.shape[1] if axis is None else self.shape[axis]
+        s = self.sum(axis=axis, dtype=rdt)
+        if axis is None:
+            with np.errstate(invalid="ignore", divide="ignore"):
+                return _deliver_scalar(rdt.type(np.true_divide(s, rdt.type(count))), out)
+        return _deliver_vector(s / count, out)
+
+    def _reduction_dtype(self, dtype, what):
+        rdt = self.dtype if dtype is None else np.dtype(dtype)
+        if rdt not in SUPPORTED_VALUE_DTYPES:
+            raise NotImplementedError(f"csr_array.{what} with dtype {rdt} is not implemented (float32/float64 only)")
+        return rdt
+
+    def _extreme(self, op, axis, out, explicit):
+        axis = self._check_reduction(axis, op)
+        if out is not None:
+            raise ValueError("Sparse min/max does not support an 'out' parameter.")
+        m, n = self.shape
+        if (m * n == 0) if axis is None else self.shape[axis] == 0:
+            raise ValueError("zero-size array to reduction operation")
+        runtime.require_cuda(f"csr_array.{op}")
+        if axis is not None:
+            return self._reduce_axis(op, axis, explicit)
+        ptr_, _, dat = self._canonical()
+        rows = _ops.csr_reduce_rows(op, ptr_, None, dat, n, explicit)
+        if explicit:
+            # an empty row has no stored value to offer; a matrix without any gives 0, as scipy does
+            rows = torch.cat([rows[ptr_[1:] > ptr_[:-1]], rows.new_zeros(1 if dat.shape[0] == 0 else 0)])
+        return self.dtype.type((rows.max() if op == "max" else rows.min()).item())
+
+    def max(self, axis=None, out=None, *, explicit=False):
+        """Largest entry of A (axis None: a numpy scalar), of every column (axis 0: a length-n CUDA tensor of A's dtype)
+        or of every row (axis 1: length m).  Implicit zeros count unless `explicit`; a NaN anywhere in a row makes that
+        row's result NaN.  Differences from scipy: along an axis the result is the dense vector, not a sparse 1-D
+        coo_array (a tensor's `.data` is the tensor itself, so `B.max(axis=0).data[B.indices]` works on both), and
+        csr_matrix, an alias of csr_array here, also returns 1-D rather than an (m, 1) matrix.  `out` is not supported
+        (ValueError), nor is a reduction over a zero-length axis.  A column reduction builds a transposed copy of A
+        once and keeps it in A's cache (with its canonical form) until A's arrays change."""
+        return self._extreme("max", axis, out, explicit)
+
+    def min(self, axis=None, out=None, *, explicit=False):
+        """Smallest entry; see `max`."""
+        return self._extreme("min", axis, out, explicit)
+
+    def _arg(self, op, axis, out, explicit):
+        axis = self._check_reduction(axis, op)
+        if out is not None:
+            raise ValueError(f"Sparse {op} does not support an 'out' parameter.")
+        m, n = self.shape
+        if axis is None and m * n == 0:
+            raise ValueError(f"Cannot apply {op} to an empty matrix.")
+        if axis is not None and self.shape[axis] == 0:
+            raise ValueError(f"Cannot apply {op} along a zero-sized dimension.")
+        if axis is None and explicit and self.nnz == 0:
+            raise ValueError(f"Cannot apply {op} to zero matrix when explicit=True.")
+        runtime.require_cuda(f"csr_array.{op}")
+        if axis is not None:
+            return self._reduce_axis(op, axis, explicit)
+        ptr_, idx, dat = self._canonical()
+        ext = "max" if op == "argmax" else "min"
+        vals = _ops.csr_reduce_rows(ext, ptr_, None, dat, n, explicit)
+        cols = _ops.csr_reduce_rows(op, ptr_, idx, dat, n, explicit)
+        # the first row (C order) holding a NaN, else the first row attaining the extreme; with `explicit`, empty rows
+        # have no candidate
+        keep = ptr_[1:] > ptr_[:-1] if explicit else torch.ones(m, dtype=torch.bool, device=vals.device)
+        rid = torch.arange(m, device=vals.device)
+        nan = keep & torch.isnan(vals)
+        ok = keep & ~nan
+        fill = torch.tensor(float("-inf") if ext == "max" else float("inf"), dtype=vals.dtype, device=vals.device)
+        masked = torch.where(ok, vals, fill)
+        g = masked.max() if ext == "max" else masked.min()
+        first_nan = torch.where(nan, rid, m).min()
+        first_hit = torch.where(ok & (vals == g), rid, m).min()
+        i = torch.where(first_nan < m, first_nan, first_hit)
+        return int((i * n + cols[i]).item())
+
+    def argmax(self, axis=None, out=None, *, explicit=False):
+        """Position of the first largest entry: for axis None the flat index i * n + j in C order (a Python int), along
+        an axis an int64 CUDA tensor of column (axis 1) or row (axis 0) indices.  Implicit zeros count unless `explicit`
+        (the first missing position stands for them).  NaN: the first NaN wins, numpy's rule on the dense row; scipy
+        1.18 instead returns the first implicit zero of a row that holds both.  With `explicit` and axis None the result
+        is still the flat index, where scipy 1.18 returns the position in its canonical data array.  `out` is not
+        supported (ValueError);
+        an empty matrix or a zero-length axis, and `explicit` on a matrix without stored entries (axis None), raise
+        ValueError.  A column reduction keeps a transposed copy of A in A's cache, as `max` does."""
+        return self._arg("argmax", axis, out, explicit)
+
+    def argmin(self, axis=None, out=None, *, explicit=False):
+        """Position of the first smallest entry; see `argmax`."""
+        return self._arg("argmin", axis, out, explicit)
+
+    def count_nonzero(self, axis=None):
+        """Number of nonzero entries of A after repeated columns are summed (axis None: a Python int), or of every column
+        (axis 0) / row (axis 1) as an int64 CUDA tensor.  Explicit zeros do not count; NaN does.  A column count keeps a
+        transposed copy of A in A's cache, as `max` does."""
+        axis = self._check_reduction(axis, "count_nonzero")
+        runtime.require_cuda("csr_array.count_nonzero")
+        if axis is None:
+            return int((self._canonical()[2] != 0).sum().item())
+        return self._reduce_axis("count_nonzero", axis)
+
+    def __abs__(self):
+        """|A| with A's structure: shares A's indptr and indices."""
+        return csr_array._from_parts(self._indptr, self._indices, self._data.abs(), self.shape)
+
+    def power(self, n, dtype=None):
+        """Elementwise power of the stored values (reference csr.py:351-360), as a new csr_array sharing A's indptr and
+        indices; the values are cast to `dtype` first when it is given.  n must be a nonzero scalar
+        (NotImplementedError otherwise: n = 0 would make every implicit zero a one)."""
+        if not np.isscalar(n):
+            raise NotImplementedError("Input is not a scalar")
+        if n == 0:
+            raise NotImplementedError("zero power is not supported as it would densify the matrix")
+        data = self._data if dtype is None else self._data.to(torch_dtype(dtype))
+        return csr_array._from_parts(self._indptr, self._indices, data**n, self.shape)
+
     def eliminate_zeros(self):
         """Remove the explicitly stored zeros (either sign), in place."""
         keep = self._data != 0
@@ -874,6 +1050,65 @@ def _column_blocks(A: csr_array, ranges) -> list:
         blocks.append(csr_array._from_parts(ip.to(_indptr_dtype(nnz)), idx[mask].contiguous(),
                                             A._data[mask].contiguous(), A.shape))
     return blocks
+
+
+def _canonical_parts(A: csr_array, rows_sorted: bool):
+    """(indptr, indices, data) of A with every row sorted and each run of a repeated column summed into its first entry
+    (row-sum kernel over the runs).  A's own arrays are never written: a sort works on clones, and a matrix already in
+    that form is returned as it is."""
+    indptr, indices, data = A._indptr, A._indices, A._data
+    if not rows_sorted and not A.has_sorted_indices:
+        indices, data = _ops.csr_sort_rows(indptr, indices.clone(), data.contiguous().clone())
+    nnz = int(data.shape[0])
+    if nnz < 2:
+        return indptr, indices, data
+    same = indices[1:] == indices[:-1]
+    starts = indptr[1:-1].to(torch.int64)
+    starts = starts[(starts > 0) & (starts < nnz)]
+    same[starts - 1] = False        # a row's first entry starts a run whatever the previous row ends with
+    if not bool(same.any()):
+        return indptr, indices, data
+    head = torch.ones(nnz, dtype=torch.bool, device=data.device)
+    head[1:] = ~same
+    heads = torch.nonzero(head).reshape(-1)
+    run_ptr = torch.cat([heads, heads.new_full((1,), nnz)])
+    merged = _ops.csr_reduce_rows("sum", run_ptr, None, data, A.shape[1])
+    runs_before = torch.zeros(nnz + 1, dtype=torch.int64, device=data.device)
+    torch.cumsum(head.to(torch.int64), 0, out=runs_before[1:])
+    return runs_before[indptr.to(torch.int64)].to(indptr.dtype), indices[heads], merged
+
+
+def _check_reduction_out(out, shape, dtype):
+    if out is None:
+        return
+    if isinstance(out, np.ndarray):
+        ok = out.dtype == dtype
+    elif isinstance(out, torch.Tensor):
+        ok = out.dtype == torch_dtype(dtype)
+    else:
+        ok = False
+    if not ok or tuple(out.shape) != tuple(shape):
+        raise ValueError(f"out must be a numpy array or torch tensor of shape {tuple(shape)} and dtype {dtype}")
+
+
+def _deliver_scalar(value, out):
+    if out is None:
+        return value
+    if isinstance(out, torch.Tensor):
+        out.fill_(float(value))
+    else:
+        out[...] = value
+    return out
+
+
+def _deliver_vector(v, out):
+    if out is None:
+        return v
+    if isinstance(out, torch.Tensor):
+        out.copy_(v)
+    else:
+        out[...] = to_host(v)
+    return out
 
 
 def _dense_rows(a, dtype):
