@@ -423,6 +423,36 @@ int         b2s_csr_reduce_rows(int op, int vt, int it, int pt, int64_t nrows, i
                                 const void* indptr, const void* indices, const void* vals, int explicit_only,
                                 void* out, void* stream);
 
+/* ---- selection: rows, columns and submatrices of a CSR matrix (csr_array.__getitem__) ------------------------------
+ * Output row t is source row rows[t] (int64, negatives count from the end; NULL: row_start + t * row_step, a slice that
+ * is never materialised).  Without a column map (col_ptr NULL, ncols_out == ncols) every entry of the row is kept.
+ * With one, col_ptr (ncols + 1, int64) and col_pos (ncols_out, int64) are a CSR matrix from source column to output
+ * positions, ascending -- b2s_coo_to_csr of (requested columns, 0..ncols_out-1) builds it -- and an entry of column c is
+ * written once per position of c.  Entries keep the source row's stored order; nothing is summed, sorted or pruned.
+ * Two passes with the same arguments and the same scratch (b2s_csr_select_scratch_bytes(nrows_out) bytes):
+ *   B2S_SELECT_COUNT : out_indptr (nrows_out + 1, int64) = the output row offsets; syncs once and returns
+ *                      info_host[4] = {nnz_out, row indices outside [-nrows, nrows), medium rows, long rows}.  When a
+ *                      row index is bad the emit pass must not run.  Reads indptr, indices (with a map), rows, col_ptr.
+ *   B2S_SELECT_EMIT  : out_indices (nnz_out, width ot) and out_vals (nnz_out values of vw = 4, 8 or 16 bytes: the
+ *                      values are only moved, so any element type of that width works).  No sync, no allocation.
+ * The outputs must not overlap the inputs or each other. */
+#define B2S_SELECT_COUNT 0
+#define B2S_SELECT_EMIT  1
+int64_t     b2s_csr_select_scratch_bytes(int64_t nrows_out);
+int         b2s_csr_select(int pass, int vw, int it, int pt, int ot, int64_t nrows, int64_t ncols, int64_t nnz,
+                           const void* indptr, const void* indices, const void* vals, int64_t nrows_out,
+                           const int64_t* rows, int64_t row_start, int64_t row_step, const int64_t* col_ptr,
+                           const int64_t* col_pos, int64_t ncols_out, int64_t* out_indptr, void* out_indices,
+                           void* out_vals, int64_t nnz_out, void* scratch, int64_t* info_host, void* stream);
+
+/* ---- element lookup: out[w] = A[ri[w], ci[w]] for k pairs (int64, negatives count from the end) ----------------------
+ * The sum of every stored entry at (i, j), added in stored order starting from the first match (scipy's
+ * csr_sample_values), or 0.  A pair outside the matrix adds 1 to the device word *bad (uint64, zeroed by the caller) and
+ * gives 0.  out (k values of vt) must not overlap the inputs.  No host sync, no allocation. */
+int         b2s_csr_lookup(int vt, int it, int pt, int64_t nrows, int64_t ncols, int64_t nnz, const void* indptr,
+                           const void* indices, const void* vals, int64_t k, const int64_t* ri, const int64_t* ci,
+                           void* out, void* bad, void* stream);
+
 /* ---- multi-GPU: NCCL communicator owned by the library (SURVEY 8b) -----------------------------------------
  * For hosts without torch.distributed (and for multi-node runs): the library binds NCCL at run time (dlopen of
  * libnccl.so.2, the one already in the process if any) and owns the communicator.  The reference uses NCCL

@@ -94,6 +94,11 @@ SIGNATURES = {
                                       c_vp]),
     "b2s_csr_reduce_rows": (c_i32, [c_i32, c_i32, c_i32, c_i32, c_i64, c_i64, c_i64, c_vp, c_vp, c_vp, c_i32, c_vp,
                                     c_vp]),
+    "b2s_csr_select_scratch_bytes": (c_i64, [c_i64]),
+    "b2s_csr_select": (c_i32, [c_i32, c_i32, c_i32, c_i32, c_i32, c_i64, c_i64, c_i64, c_vp, c_vp, c_vp, c_i64, c_vp,
+                               c_i64, c_i64, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp]),
+    "b2s_csr_lookup": (c_i32, [c_i32, c_i32, c_i32, c_i64, c_i64, c_i64, c_vp, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp,
+                               c_vp, c_vp]),
     "b2s_comm_nccl_version": (c_i32, []),
     "b2s_comm_unique_id": (c_i32, [c_vp]),
     "b2s_comm_init": (c_i32, [c_i32, c_i32, c_vp, ctypes.POINTER(c_vp)]),

@@ -484,6 +484,78 @@ def csr_reduce_rows(op: str, indptr, indices, data, ncols: int, explicit: bool =
     return out
 
 
+def csr_column_map(cols, ncols: int):
+    """The column map of a column selection through b2s_coo_to_csr: (col_ptr, col_pos, bad), an int64 CSR matrix from
+    source column to the output positions (ascending) that request it, and the number of requested columns outside
+    [-ncols, ncols).  `cols` is an int64 device tensor; negative entries count from the end.  Syncs once."""
+    _chk_dev(cols)
+    k = int(cols.shape[0])
+    dev = cols.device
+    cols = torch.where(cols < 0, cols + ncols, cols).contiguous()
+    pos = torch.arange(k, dtype=torch.int64, device=dev)
+    dummy = torch.zeros(k, dtype=torch.float32, device=dev)      # b2s_coo_to_csr moves values; these are not read back
+    col_ptr = torch.empty(ncols + 1, dtype=torch.int64, device=dev)
+    col_pos = torch.empty(k, dtype=torch.int64, device=dev)
+    out_vals = torch.empty(k, dtype=torch.float32, device=dev)
+    scratch = torch.empty(int(L.b2s_convert_scratch_bytes(ncols, _lib.I64)), dtype=torch.uint8, device=dev)
+    bad = _lib.c_i64(0)
+    _lib.check(L.b2s_coo_to_csr(_lib.F32, _lib.I64, _lib.I64, ncols, k, ptr(cols), ptr(pos), ptr(dummy), ptr(col_ptr),
+                                ptr(col_pos), ptr(out_vals), ptr(scratch), ctypes.byref(bad), _stream()),
+               "b2s_coo_to_csr")
+    return col_ptr, col_pos, int(bad.value)
+
+
+def csr_select(indptr, indices, data, shape, nrows_out: int, rows=None, row_start: int = 0, row_step: int = 1,
+               col_map=None, ncols_out=None, out_index_dtype=torch.int32):
+    """Rows and columns of a CSR matrix through the two passes of b2s_csr_select.  Output row t is source row rows[t]
+    (an int64 device tensor; negatives count from the end) or row_start + t * row_step; col_map = (col_ptr, col_pos) of
+    `csr_column_map`, or None for every column.  Returns (indptr int64, indices of out_index_dtype, data, bad): with
+    bad > 0 row indices outside the matrix, indices and data are None.  Syncs once."""
+    _chk_dev(indptr, indices, data, rows)
+    nrows, ncols = shape
+    dev = data.device
+    indices, data = indices.contiguous(), data.contiguous()
+    col_ptr, col_pos = col_map if col_map is not None else (None, None)
+    if col_map is None:
+        ncols_out = ncols
+    if rows is not None:
+        rows = rows.contiguous()
+    vw = data.element_size()
+    it, pt, ot = idx_code(indices.dtype), idx_code(indptr.dtype), idx_code(out_index_dtype)
+    st = _stream()
+    scratch = torch.empty(int(L.b2s_csr_select_scratch_bytes(nrows_out)), dtype=torch.uint8, device=dev)
+    out_ptr = torch.empty(nrows_out + 1, dtype=torch.int64, device=dev)
+    info = (_lib.c_i64 * 4)()
+    args = (nrows, ncols, int(data.shape[0]), ptr(indptr), ptr(indices), ptr(data), nrows_out, ptr(rows), row_start,
+            row_step, ptr(col_ptr), ptr(col_pos), ncols_out, ptr(out_ptr))
+    _lib.check(L.b2s_csr_select(0, vw, it, pt, ot, *args, None, None, 0, ptr(scratch), info, st), "b2s_csr_select")
+    nnz_out, bad = int(info[0]), int(info[1])
+    if bad:
+        return out_ptr, None, None, bad
+    out_idx = torch.empty(nnz_out, dtype=out_index_dtype, device=dev)
+    out_val = torch.empty(nnz_out, dtype=data.dtype, device=dev)
+    _lib.check(L.b2s_csr_select(1, vw, it, pt, ot, *args, ptr(out_idx), ptr(out_val), nnz_out, ptr(scratch), None, st),
+               "b2s_csr_select")
+    return out_ptr, out_idx, out_val, 0
+
+
+def csr_lookup(indptr, indices, data, shape, ri, ci):
+    """out[w] = A[ri[w], ci[w]] (int64 device tensors; negatives count from the end) through b2s_csr_lookup: the sum of
+    the stored entries there in stored order, or 0.  Returns (out, bad) with bad a one-element int64 device tensor
+    counting the pairs outside the matrix; nothing syncs."""
+    _chk_dev(indptr, indices, data, ri, ci)
+    nrows, ncols = shape
+    k = int(ri.shape[0])
+    ri, ci, indices, data = ri.contiguous(), ci.contiguous(), indices.contiguous(), data.contiguous()
+    out = torch.empty(k, dtype=data.dtype, device=data.device)
+    bad = torch.zeros(1, dtype=torch.int64, device=data.device)
+    _lib.check(L.b2s_csr_lookup(vt_code(data.dtype), idx_code(indices.dtype), idx_code(indptr.dtype), nrows, ncols,
+                                int(data.shape[0]), ptr(indptr), ptr(indices), ptr(data), k, ptr(ri), ptr(ci), ptr(out),
+                                ptr(bad), _stream()),
+               "b2s_csr_lookup")
+    return out, bad
+
+
 def spgemm_row_work(a_indptr, a_indices, b_indptr) -> torch.Tensor:
     """Products per row of A @ B (int64 device tensor of len m): the chunk planner's measure of work / output size."""
     _chk_dev(a_indptr, a_indices, b_indptr)

@@ -997,6 +997,73 @@ class csr_array:
         self._indices, self._data = _ops.csr_sort_rows(self._indptr, self._indices.clone(), self._data.clone())
         self._cache.clear()
 
+    # -- indexing (scipy csr_matrix semantics; csrc/index.cu) ----------------------------------------------------------
+    def __getitem__(self, key):
+        """scipy-style indexing on the device.
+
+        * `A[i, j]`, two integers: the numpy scalar sum of the entries stored at (i, j), added in stored order, or 0.
+        * `A[I, J]`, two 1-D index arrays of one length k: the k element values, numpy for host indices and a CUDA tensor
+          for CUDA indices, as `dot` returns.
+        * `A[r]`, `A[r, :]`, `A[:, c]`, `A[r, c]`, `A[..., c]` with r and c each an int, a slice (any step), a 1-D integer
+          array (any order, repeats, negatives) or a 1-D boolean mask, not both arrays; and `A[np.ix_(I, J)]`: a new
+          csr_array of the outer selection.  As in scipy's csr_matrix (csr_matrix is an alias of csr_array here), an
+          integer keeps its axis with length 1; scipy's csr_array would return a 1-D coo_array, a type this library
+          does not have.
+        Entries keep the source row's stored order; an entry whose column is requested r times appears r times, output
+        columns ascending; duplicates and explicit zeros are kept.  The result holds new arrays; A is not modified.
+        Index arrays may be lists, numpy arrays or tensors on either side.  Out-of-range indices, a mask of the wrong
+        length, too many indices and None raise IndexError, as do float index arrays (scipy truncates them; numpy
+        refuses them).  Other 2-D index arrays raise NotImplementedError, and so do lookups on data other than
+        float32 / float64 (selections move values of any 4-, 8- or 16-byte type).  A selection syncs once (twice with
+        a column selection: the column map is built first); CUDA row and column indices are checked on the device."""
+        kind, R, C = _index_key(key, self.shape)
+        if kind in ("element", "points"):
+            if self.dtype not in SUPPORTED_VALUE_DTYPES:
+                raise NotImplementedError(f"element lookup for dtype {self.dtype} is not implemented (float32/float64 only)")
+            runtime.require_cuda("csr_array.__getitem__")
+            dev = self.device
+            on_device = kind == "points" and any(isinstance(a, torch.Tensor) for a in (R, C))
+            ri, ci = (_index_tensor(np.asarray([a]) if kind == "element" else a, dev) for a in (R, C))
+            out, bad = _ops.csr_lookup(self._indptr, self._indices, self._data, self.shape, ri, ci)
+            if on_device:
+                if int(bad.item()):
+                    raise IndexError(f"{int(bad.item())} index pairs out of range for shape {self.shape}")
+                return out
+            res = to_host(out)
+            return self.dtype.type(res[0]) if kind == "element" else res
+        if self._data.element_size() not in (4, 8, 16):
+            raise NotImplementedError(f"selection for dtype {self.dtype} is not implemented (4-, 8- or 16-byte values)")
+        runtime.require_cuda("csr_array.__getitem__")
+        return self._select(R, C)
+
+    def _select(self, R, C):
+        """The outer selection of `_index_key`'s row and column selections (each ("slice", start, step, count) or
+        ("array", int64 indices))."""
+        m, n = self.shape
+        dev = self.device
+        rows, start, step = None, 0, 1
+        if R[0] == "slice":
+            start, step, nout = R[1], R[2], R[3]
+        else:
+            rows = _index_tensor(R[1], dev)
+            nout = int(rows.shape[0])
+        col_map, ncols_out = None, n
+        if C != ("slice", 0, 1, n):
+            if C[0] == "slice":
+                cols = torch.arange(C[1], C[1] + C[2] * C[3], C[2], dtype=torch.int64, device=dev)
+            else:
+                cols = _index_tensor(C[1], dev)
+            ncols_out = int(cols.shape[0])
+            col_ptr, col_pos, bad = _ops.csr_column_map(cols, n)
+            if bad:
+                raise IndexError(f"{bad} column indices out of range for {n} columns")
+            col_map = (col_ptr, col_pos)
+        ptr_, idx, dat, bad = _ops.csr_select(self._indptr, self._indices, self._data, self.shape, nout, rows, start,
+                                              step, col_map, ncols_out, _index_dtype(ncols_out - 1))
+        if bad:
+            raise IndexError(f"{bad} row indices out of range for {m} rows")
+        return csr_array._from_parts(ptr_.to(_indptr_dtype(int(idx.shape[0]))), idx, dat, (nout, ncols_out))
+
     def balance(self):
         """No-op on a single device; kept for API parity (reference base.py:198-282 re-tiles the rows by
         nnz; the multi-GPU row plan lives in dist.py)."""
@@ -1076,6 +1143,104 @@ def _canonical_parts(A: csr_array, rows_sorted: bool):
     runs_before = torch.zeros(nnz + 1, dtype=torch.int64, device=data.device)
     torch.cumsum(head.to(torch.int64), 0, out=runs_before[1:])
     return runs_before[indptr.to(torch.int64)].to(indptr.dtype), indices[heads], merged
+
+
+def _axis_index(x, n: int):
+    """One axis of an index key, for an axis of length n: ("int", i) with 0 <= i < n, ("slice", start, step, count), or
+    ("array", indices) -- an int64 numpy array wrapped into [0, n), or an int64 CUDA tensor left as given (the kernels
+    wrap and check it).  Masks become the positions of their True entries."""
+    if isinstance(x, (bool, np.bool_)):
+        raise IndexError("a boolean scalar is not a valid index")
+    if isinstance(x, (int, np.integer)):
+        i = int(x)
+        if not -n <= i < n:
+            raise IndexError(f"index ({i}) out of range for an axis of length {n}")
+        return ("int", i + n if i < 0 else i)
+    if isinstance(x, slice):
+        start, stop, step = x.indices(n)        # ValueError for a zero step, as scipy
+        count = len(range(start, stop, step))
+        return ("slice", start if count else 0, step, count)
+    if isinstance(x, torch.Tensor) and x.is_cuda:
+        if x.ndim == 0:
+            return _axis_index(x.item(), n)
+        if x.ndim != 1:
+            raise NotImplementedError("index arrays must be 1-D, or the pair np.ix_ makes")
+        if x.dtype == torch.bool:
+            if x.shape[0] != n:
+                raise IndexError(f"boolean index of length {x.shape[0]} for an axis of length {n}")
+            return ("array", torch.nonzero(x).reshape(-1))
+        if not _is_integer_dtype(x.dtype):
+            raise IndexError(f"arrays used as indices must be of integer (or boolean) type, got {x.dtype}")
+        return ("array", x.to(torch.int64))
+    a = x.numpy() if isinstance(x, torch.Tensor) else np.asarray(x)
+    if a.ndim == 0:
+        if a.dtype.kind in "iu":
+            return _axis_index(int(a), n)
+        raise IndexError(f"only integers, slices, ellipsis and integer or boolean arrays are valid indices, got {x!r}")
+    if a.ndim != 1:
+        raise NotImplementedError("index arrays must be 1-D, or the pair np.ix_ makes")
+    if a.size == 0 and a.dtype.kind == "f":
+        a = a.astype(np.int64)               # [] is an empty index
+    if a.dtype.kind == "b":
+        if a.size != n:
+            raise IndexError(f"boolean index of length {a.size} for an axis of length {n}")
+        return ("array", np.flatnonzero(a).astype(np.int64))
+    if a.dtype.kind not in "iu":
+        raise IndexError(f"arrays used as indices must be of integer (or boolean) type, got {a.dtype}")
+    a = a.astype(np.int64)
+    if a.size and (a.min() < -n or a.max() >= n):
+        bad = a[(a < -n) | (a >= n)][0]
+        raise IndexError(f"index ({bad}) out of range for an axis of length {n}")
+    return ("array", np.where(a < 0, a + n, a))
+
+
+def _ndim(x):
+    return x.ndim if isinstance(x, (np.ndarray, torch.Tensor)) else np.ndim(x) if isinstance(x, list) else 0
+
+
+def _index_key(key, shape):
+    """The host half of `csr_array.__getitem__`, touching no device: ("element", i, j) for two integers, ("points", I,
+    J) for two 1-D index arrays of one length, or ("outer", R, C) with R and C each ("slice", start, step, count) or
+    ("array", indices) (an integer becomes a slice of one).  Raises what scipy raises for a malformed key (see
+    `csr_array.__getitem__`)."""
+    m, n = shape
+    parts = list(key) if isinstance(key, tuple) else [key]
+    if len(parts) == 2 and all(_ndim(p) == 2 for p in parts):
+        r, c = (p if isinstance(p, (np.ndarray, torch.Tensor)) else np.asarray(p) for p in parts)
+        if r.shape[1] == 1 and c.shape[0] == 1:                  # np.ix_(I, J)
+            R, C = _axis_index(r.reshape(-1), m), _axis_index(c.reshape(-1), n)
+            return ("outer", R, C)
+        raise NotImplementedError("2-D index arrays other than the pair np.ix_ makes are not supported")
+    if any(p is None for p in parts):
+        raise IndexError("None (newaxis) is not supported in sparse indexing")
+    ell = [k for k, p in enumerate(parts) if p is Ellipsis]
+    if len(ell) > 1:
+        raise IndexError("an index can only have a single ellipsis ('...')")
+    if ell:
+        k = ell[0]
+        fill = 2 - (len(parts) - 1)
+        if fill < 0:
+            raise IndexError("too many indices for a 2-D sparse array")
+        parts = parts[:k] + [slice(None)] * fill + parts[k + 1:]
+    if len(parts) > 2:
+        raise IndexError("too many indices for a 2-D sparse array")
+    parts += [slice(None)] * (2 - len(parts))
+    R, C = _axis_index(parts[0], m), _axis_index(parts[1], n)
+    if R[0] == "int" and C[0] == "int":
+        return ("element", R[1], C[1])
+    if R[0] == "array" and C[0] == "array":
+        if R[1].shape[0] != C[1].shape[0]:
+            raise IndexError(f"shape mismatch: index arrays of lengths {R[1].shape[0]} and {C[1].shape[0]}")
+        return ("points", R[1], C[1])
+    as_sel = lambda s: ("slice", s[1], 1, 1) if s[0] == "int" else s  # noqa: E731
+    return ("outer", as_sel(R), as_sel(C))
+
+
+def _index_tensor(a, device) -> torch.Tensor:
+    """An int64 index array (numpy or tensor) as a contiguous int64 tensor on `device`."""
+    if isinstance(a, torch.Tensor):
+        return a.to(device=device, dtype=torch.int64).contiguous()
+    return torch.from_numpy(np.ascontiguousarray(a, dtype=np.int64)).to(device)
 
 
 def _check_reduction_out(out, shape, dtype):
