@@ -24,6 +24,10 @@
  *    pt: indptr width 0=int32 1=int64  (reference: util/dispatch.h:23-74);
  *  - CSR is scipy-style: indptr[nrows+1], indices[nnz], vals[nnz].  The reference's
  *    Rect<1> `pos` {lo,hi} (sparse/csr.py:186-203) is indptr[i], indptr[i+1]-1.
+ *  - every entry point that takes `it` and `pt` rejects with B2S_EINVAL: an `it` or `pt`
+ *    other than 0 / 1, a negative nrows, ncols or nnz, and an int32 indptr (pt = 0) with
+ *    nnz >= 2^31-1.  A bound on nrows is per entry point: the kernels that number rows
+ *    with 32-bit ids (SpMV, SpMM, SDDMM, tropical SpMV, row reductions) need nrows < 2^31-1.
  */
 #ifndef B200SPARSE_H
 #define B200SPARSE_H

@@ -17,6 +17,14 @@ void set_error(const char* fmt, ...) {
   va_end(ap);
 }
 
+int check_csr(int it, int pt, int64_t nrows, int64_t ncols, int64_t nnz) {
+  B2S_CHECK_ARG(it == B2S_I32 || it == B2S_I64, "bad index type code %d", it);
+  B2S_CHECK_ARG(pt == B2S_I32 || pt == B2S_I64, "bad indptr type code %d", pt);
+  B2S_CHECK_ARG(nrows >= 0 && ncols >= 0 && nnz >= 0, "negative dimension");
+  B2S_CHECK_ARG(pt == B2S_I64 || nnz < 2147483647LL, "int32 indptr cannot address nnz >= 2^31-1");
+  return B2S_OK;
+}
+
 int get_props(DeviceProps* out) {
   static DeviceProps cache[64];
   static bool have[64] = {false};

@@ -31,6 +31,18 @@ void set_error(const char* fmt, ...);
 
 #define B2S_LAUNCH_CHECK() B2S_CUDA(cudaGetLastError())
 
+// The CSR operand contract of every entry point that takes `it` and `pt` (include/b200sparse.h, Conventions): known
+// index and indptr type codes, no negative size, and an int32 indptr only below 2^31-1 entries.  Entry points without
+// an ncols or nnz argument pass 0.  Returns B2S_OK, or B2S_EINVAL with the message set.
+int check_csr(int it, int pt, int64_t nrows, int64_t ncols, int64_t nnz);
+
+// true when the byte ranges [p, p + bytes) and [q, q + qbytes) do not intersect (an empty or NULL range never does)
+inline bool disjoint(const void* p, int64_t bytes, const void* q, int64_t qbytes) {
+  if (p == nullptr || q == nullptr || bytes <= 0 || qbytes <= 0) return true;
+  const uintptr_t a = (uintptr_t)p, b = (uintptr_t)q;
+  return a + (uintptr_t)bytes <= b || b + (uintptr_t)qbytes <= a;
+}
+
 // ---- ABI type codes to C++ types ----------------------------------------------------
 // Each calls `f` with a value of the type a code names (`using V = decltype(v);` recovers it) and returns f's int.  An
 // unknown code sets an error and returns B2S_EINVAL; entry points check their codes first, with their own messages.

@@ -269,10 +269,9 @@ int b2s_coo_to_csr(int vt, int it, int pt, int64_t nrows, int64_t nnz, const voi
                    const void* vals, void* indptr, void* indices, void* vals_out, void* scratch, int64_t* bad_host,
                    void* stream) {
   B2S_CHECK_ARG(vt == B2S_F32 || vt == B2S_F64, "bad value type code %d", vt);
-  B2S_CHECK_ARG((it == B2S_I32 || it == B2S_I64) && (pt == B2S_I32 || pt == B2S_I64), "bad index type codes");
-  B2S_CHECK_ARG(nrows >= 0 && nnz >= 0 && indptr && scratch, "bad arguments");
+  if (int rc = check_csr(it, pt, nrows, 0, nnz)) return rc;
+  B2S_CHECK_ARG(indptr && scratch, "indptr / scratch is NULL");
   B2S_CHECK_ARG(nnz == 0 || (rows && cols && vals && indices && vals_out), "NULL array with nnz > 0");
-  B2S_CHECK_ARG(pt == B2S_I64 || nnz < 2147483647LL, "int32 indptr cannot address nnz >= 2^31-1");
   cudaStream_t st = (cudaStream_t)stream;
   unsigned char* sc = (unsigned char*)scratch;
   return with_value_type(vt, [&](auto v) {
@@ -291,8 +290,8 @@ int b2s_csr_transpose(int vt, int it, int pt, int64_t nrows, int64_t ncols, int6
                       const void* indices, const void* vals, void* t_indptr, void* t_indices, void* t_vals,
                       void* scratch, void* stream) {
   B2S_CHECK_ARG(vt == B2S_F32 || vt == B2S_F64, "bad value type code %d", vt);
-  B2S_CHECK_ARG((it == B2S_I32 || it == B2S_I64) && (pt == B2S_I32 || pt == B2S_I64), "bad index type codes");
-  B2S_CHECK_ARG(nrows >= 0 && ncols >= 0 && nnz >= 0 && indptr && t_indptr && scratch, "bad arguments");
+  if (int rc = check_csr(it, pt, nrows, ncols, nnz)) return rc;
+  B2S_CHECK_ARG(indptr && t_indptr && scratch, "indptr / t_indptr / scratch is NULL");
   B2S_CHECK_ARG(nnz == 0 || (indices && vals && t_indices && t_vals), "NULL array with nnz > 0");
   cudaStream_t st = (cudaStream_t)stream;
   unsigned char* sc = (unsigned char*)scratch;
@@ -315,8 +314,8 @@ int b2s_csr_transpose(int vt, int it, int pt, int64_t nrows, int64_t ncols, int6
 int b2s_csr_sort_rows(int vt, int it, int pt, int64_t nrows, int64_t nnz, const void* indptr, void* indices,
                       void* vals, void* scratch, void* stream) {
   B2S_CHECK_ARG(vt == B2S_F32 || vt == B2S_F64, "bad value type code %d", vt);
-  B2S_CHECK_ARG((it == B2S_I32 || it == B2S_I64) && (pt == B2S_I32 || pt == B2S_I64), "bad index type codes");
-  B2S_CHECK_ARG(nrows >= 0 && nnz >= 0 && indptr && scratch, "bad arguments");
+  if (int rc = check_csr(it, pt, nrows, 0, nnz)) return rc;
+  B2S_CHECK_ARG(indptr && scratch, "indptr / scratch is NULL");
   B2S_CHECK_ARG(nnz == 0 || (indices && vals), "NULL array with nnz > 0");
   DeviceProps pr;
   if (int rc = get_props(&pr)) return rc;

@@ -344,8 +344,7 @@ int b2s_csr_binop_symbolic(int op, int it, int pt, int64_t m, int64_t n, const v
                            const void* b_indptr, const void* b_indices, int64_t* c_indptr, int64_t* info_host,
                            void* scratch, void* stream) {
   B2S_CHECK_ARG(op == B2S_EW_ADD || op == B2S_EW_SUB || op == B2S_EW_MUL, "bad op code %d", op);
-  B2S_CHECK_ARG((it == B2S_I32 || it == B2S_I64) && (pt == B2S_I32 || pt == B2S_I64), "bad index type codes");
-  B2S_CHECK_ARG(m >= 0 && n >= 0, "negative dimension");
+  if (int rc = check_csr(it, pt, m, n, 0)) return rc;
   B2S_CHECK_ARG(a_indptr && b_indptr && c_indptr && info_host && scratch, "NULL pointer argument");
   DeviceProps pr;
   if (int rc = get_props(&pr)) return rc;
@@ -383,8 +382,7 @@ int b2s_csr_binop_numeric(int op, int vt, int it, int pt, int64_t m, int64_t n, 
                           void* stream) {
   B2S_CHECK_ARG(op == B2S_EW_ADD || op == B2S_EW_SUB || op == B2S_EW_MUL, "bad op code %d", op);
   B2S_CHECK_ARG(vt == B2S_F32 || vt == B2S_F64, "bad value type code %d", vt);
-  B2S_CHECK_ARG((it == B2S_I32 || it == B2S_I64) && (pt == B2S_I32 || pt == B2S_I64), "bad index type codes");
-  B2S_CHECK_ARG(m >= 0 && n >= 0, "negative dimension");
+  if (int rc = check_csr(it, pt, m, n, 0)) return rc;
   B2S_CHECK_ARG(a_indptr && b_indptr && c_indptr && scratch, "NULL pointer argument");
   if (m == 0) return B2S_OK;
   DeviceProps pr;
@@ -403,9 +401,9 @@ int b2s_csr_binop_numeric(int op, int vt, int it, int pt, int64_t m, int64_t n, 
 int b2s_csr_scale(int vt, int it, int pt, int64_t m, int64_t n, int64_t nnz, int mode, const void* indptr,
                   const void* indices, const void* vals, const void* d, int64_t ldd, void* out_vals, void* stream) {
   B2S_CHECK_ARG(vt == B2S_F32 || vt == B2S_F64, "bad value type code %d", vt);
-  B2S_CHECK_ARG((it == B2S_I32 || it == B2S_I64) && (pt == B2S_I32 || pt == B2S_I64), "bad index type codes");
+  if (int rc = check_csr(it, pt, m, n, nnz)) return rc;
   B2S_CHECK_ARG(mode == B2S_SCALE_ROWS || mode == B2S_SCALE_COLS || mode == B2S_SCALE_DENSE, "bad scale mode %d", mode);
-  B2S_CHECK_ARG(m >= 0 && n >= 0 && nnz >= 0 && indptr, "bad arguments");
+  B2S_CHECK_ARG(indptr, "indptr is NULL");
   B2S_CHECK_ARG(mode != B2S_SCALE_DENSE || ldd >= n, "leading dimension %lld < ncols", (long long)ldd);
   B2S_CHECK_ARG(nnz == 0 || (indices && vals && d && out_vals), "NULL array with nnz > 0");
   if (m == 0 || nnz == 0) return B2S_OK;

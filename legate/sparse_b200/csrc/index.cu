@@ -398,13 +398,6 @@ static int ix_emit(const DeviceProps& pr, const SelectArgs& a, unsigned char* sc
   return B2S_OK;
 }
 
-// true when the byte ranges [p, p + bytes) and [q, q + qbytes) do not intersect (an empty or NULL range never does)
-inline bool ix_apart(const void* p, int64_t bytes, const void* q, int64_t qbytes) {
-  if (p == nullptr || q == nullptr || bytes <= 0 || qbytes <= 0) return true;
-  const uintptr_t a = (uintptr_t)p, b = (uintptr_t)q;
-  return a + (uintptr_t)bytes <= b || b + (uintptr_t)qbytes <= a;
-}
-
 }  // namespace b2s
 
 using namespace b2s;
@@ -423,12 +416,9 @@ int b2s_csr_select(int pass, int vw, int it, int pt, int ot, int64_t nrows, int6
                    void* scratch, int64_t* info_host, void* stream) {
   B2S_CHECK_ARG(pass == B2S_SELECT_COUNT || pass == B2S_SELECT_EMIT, "bad pass %d", pass);
   B2S_CHECK_ARG(vw == 4 || vw == 8 || vw == 16, "bad value width %d", vw);
-  B2S_CHECK_ARG(it == B2S_I32 || it == B2S_I64, "bad index type code %d", it);
-  B2S_CHECK_ARG(pt == B2S_I32 || pt == B2S_I64, "bad indptr type code %d", pt);
+  if (int rc = check_csr(it, pt, nrows, ncols, nnz)) return rc;
   B2S_CHECK_ARG(ot == B2S_I32 || ot == B2S_I64, "bad output index type code %d", ot);
-  B2S_CHECK_ARG(nrows >= 0 && ncols >= 0 && nnz >= 0 && nrows_out >= 0 && ncols_out >= 0 && nnz_out >= 0,
-                "negative dimension");
-  B2S_CHECK_ARG(pt == B2S_I64 || nnz < 2147483647LL, "int32 indptr cannot address nnz >= 2^31-1");
+  B2S_CHECK_ARG(nrows_out >= 0 && ncols_out >= 0 && nnz_out >= 0, "negative dimension");
   B2S_CHECK_ARG(ot == B2S_I64 || ncols_out <= 2147483648LL, "int32 output indices cannot hold %lld columns",
                 (long long)ncols_out);
   B2S_CHECK_ARG(col_ptr != nullptr || ncols_out == ncols, "without a column map every column is kept");
@@ -450,16 +440,16 @@ int b2s_csr_select(int pass, int vw, int it, int pt, int ot, int64_t nrows, int6
                                 col_ptr ? (ncols + 1) * 8 : 0, col_pos ? ncols_out * 8 : 0};
     const char* names[] = {"indptr", "indices", "vals", "rows", "col_ptr", "col_pos"};
     for (int k = 0; k < 6; k++) {
-      B2S_CHECK_ARG(ix_apart(out_indptr, ptr_bytes, ins[k], in_bytes[k]), "out_indptr overlaps %s", names[k]);
+      B2S_CHECK_ARG(disjoint(out_indptr, ptr_bytes, ins[k], in_bytes[k]), "out_indptr overlaps %s", names[k]);
       if (pass == B2S_SELECT_EMIT) {
-        B2S_CHECK_ARG(ix_apart(out_indices, nnz_out * osz, ins[k], in_bytes[k]), "out_indices overlaps %s", names[k]);
-        B2S_CHECK_ARG(ix_apart(out_vals, nnz_out * vw, ins[k], in_bytes[k]), "out_vals overlaps %s", names[k]);
+        B2S_CHECK_ARG(disjoint(out_indices, nnz_out * osz, ins[k], in_bytes[k]), "out_indices overlaps %s", names[k]);
+        B2S_CHECK_ARG(disjoint(out_vals, nnz_out * vw, ins[k], in_bytes[k]), "out_vals overlaps %s", names[k]);
       }
     }
     if (pass == B2S_SELECT_EMIT) {
-      B2S_CHECK_ARG(ix_apart(out_indices, nnz_out * osz, out_vals, nnz_out * vw), "out_indices overlaps out_vals");
-      B2S_CHECK_ARG(ix_apart(out_indptr, ptr_bytes, out_indices, nnz_out * osz), "out_indptr overlaps out_indices");
-      B2S_CHECK_ARG(ix_apart(out_indptr, ptr_bytes, out_vals, nnz_out * vw), "out_indptr overlaps out_vals");
+      B2S_CHECK_ARG(disjoint(out_indices, nnz_out * osz, out_vals, nnz_out * vw), "out_indices overlaps out_vals");
+      B2S_CHECK_ARG(disjoint(out_indptr, ptr_bytes, out_indices, nnz_out * osz), "out_indptr overlaps out_indices");
+      B2S_CHECK_ARG(disjoint(out_indptr, ptr_bytes, out_vals, nnz_out * vw), "out_indptr overlaps out_vals");
     }
   }
   DeviceProps pr;
@@ -492,10 +482,8 @@ int b2s_csr_lookup(int vt, int it, int pt, int64_t nrows, int64_t ncols, int64_t
                    const void* indices, const void* vals, int64_t k, const int64_t* ri, const int64_t* ci, void* out,
                    void* bad, void* stream) {
   B2S_CHECK_ARG(vt == B2S_F32 || vt == B2S_F64, "bad value type code %d", vt);
-  B2S_CHECK_ARG(it == B2S_I32 || it == B2S_I64, "bad index type code %d", it);
-  B2S_CHECK_ARG(pt == B2S_I32 || pt == B2S_I64, "bad indptr type code %d", pt);
-  B2S_CHECK_ARG(nrows >= 0 && ncols >= 0 && nnz >= 0 && k >= 0, "negative dimension");
-  B2S_CHECK_ARG(pt == B2S_I64 || nnz < 2147483647LL, "int32 indptr cannot address nnz >= 2^31-1");
+  if (int rc = check_csr(it, pt, nrows, ncols, nnz)) return rc;
+  B2S_CHECK_ARG(k >= 0, "negative dimension");
   if (k == 0) return B2S_OK;
   B2S_CHECK_ARG(ri != nullptr && ci != nullptr, "row/column index arrays NULL with k > 0");
   B2S_CHECK_ARG(out != nullptr, "out is NULL");
@@ -508,7 +496,7 @@ int b2s_csr_lookup(int vt, int it, int pt, int64_t nrows, int64_t ncols, int64_t
     const int64_t in_bytes[] = {(nrows + 1) * psz, nnz * isz, nnz * vsz, k * 8, k * 8, 8};
     const char* names[] = {"indptr", "indices", "vals", "row indices", "column indices", "bad"};
     for (int q = 0; q < 6; q++)
-      B2S_CHECK_ARG(ix_apart(out, k * vsz, ins[q], in_bytes[q]), "out overlaps %s", names[q]);
+      B2S_CHECK_ARG(disjoint(out, k * vsz, ins[q], in_bytes[q]), "out overlaps %s", names[q]);
   }
   cudaStream_t st = (cudaStream_t)stream;
   return with_value_type(vt, [&](auto v) {

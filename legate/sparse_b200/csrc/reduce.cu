@@ -228,11 +228,8 @@ int b2s_csr_reduce_rows(int op, int vt, int it, int pt, int64_t nrows, int64_t n
                         void* stream) {
   B2S_CHECK_ARG(op >= B2S_REDUCE_SUM && op <= B2S_REDUCE_COUNT_NONZERO, "bad reduction code %d", op);
   B2S_CHECK_ARG(vt == B2S_F32 || vt == B2S_F64, "bad value type code %d", vt);
-  B2S_CHECK_ARG(it == B2S_I32 || it == B2S_I64, "bad index type code %d", it);
-  B2S_CHECK_ARG(pt == B2S_I32 || pt == B2S_I64, "bad indptr type code %d", pt);
-  B2S_CHECK_ARG(nrows >= 0 && ncols >= 0 && nnz >= 0, "negative dimension");
+  if (int rc = check_csr(it, pt, nrows, ncols, nnz)) return rc;
   B2S_CHECK_ARG(nrows < 2147483647LL, "nrows >= 2^31-1 is not supported");
-  B2S_CHECK_ARG(pt == B2S_I64 || nnz < 2147483647LL, "int32 indptr cannot address nnz >= 2^31-1");
   if (nrows == 0) return B2S_OK;
   const bool arg = op == B2S_REDUCE_ARGMAX || op == B2S_REDUCE_ARGMIN;
   B2S_CHECK_ARG(indptr != nullptr, "indptr is NULL");
@@ -241,17 +238,13 @@ int b2s_csr_reduce_rows(int op, int vt, int it, int pt, int64_t nrows, int64_t n
   B2S_CHECK_ARG(nnz == 0 || vals != nullptr, "vals NULL with nnz > 0");
   B2S_CHECK_ARG(!arg || nnz == 0 || indices != nullptr, "indices NULL with nnz > 0");
   {
-    // byte ranges [lo, hi) the kernel reads, against the one it writes
+    // the byte ranges the kernel reads, against the one it writes
     const int64_t vsz = vt == B2S_F64 ? 8 : 4, isz = it == B2S_I64 ? 8 : 4, psz = pt == B2S_I64 ? 8 : 4;
     const bool int_out = arg || op == B2S_REDUCE_COUNT_NONZERO;
-    const uintptr_t olo = (uintptr_t)out, ohi = olo + (uintptr_t)(nrows * (int_out ? 8 : vsz));
-    auto apart = [&](const void* p, int64_t bytes) {
-      const uintptr_t lo = (uintptr_t)p, hi = lo + (uintptr_t)bytes;
-      return p == nullptr || bytes == 0 || hi <= olo || ohi <= lo;
-    };
-    B2S_CHECK_ARG(apart(vals, nnz * vsz), "out overlaps vals");
-    B2S_CHECK_ARG(apart(indices, nnz * isz), "out overlaps indices");
-    B2S_CHECK_ARG(apart(indptr, (nrows + 1) * psz), "out overlaps indptr");
+    const int64_t obytes = nrows * (int_out ? 8 : vsz);
+    B2S_CHECK_ARG(disjoint(out, obytes, vals, nnz * vsz), "out overlaps vals");
+    B2S_CHECK_ARG(disjoint(out, obytes, indices, nnz * isz), "out overlaps indices");
+    B2S_CHECK_ARG(disjoint(out, obytes, indptr, (nrows + 1) * psz), "out overlaps indptr");
   }
   cudaStream_t st = (cudaStream_t)stream;
   return with_value_type(vt, [&](auto v) {

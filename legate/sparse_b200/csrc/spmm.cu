@@ -431,11 +431,9 @@ int b2s_spmm_csr(int vt, int it, int pt, int64_t nrows, int64_t ncols, int64_t n
                  const void* indices, const void* vals, const void* X, int64_t ldx, void* Y, int64_t ldy,
                  void* stream) {
   B2S_CHECK_ARG(vt == B2S_F32 || vt == B2S_F64, "bad value type code %d", vt);
-  B2S_CHECK_ARG(it == B2S_I32 || it == B2S_I64, "bad index type code %d", it);
-  B2S_CHECK_ARG(pt == B2S_I32 || pt == B2S_I64, "bad indptr type code %d", pt);
-  B2S_CHECK_ARG(nrows >= 0 && ncols >= 0 && nnz >= 0 && k >= 0, "negative dimension");
+  if (int rc = check_csr(it, pt, nrows, ncols, nnz)) return rc;
+  B2S_CHECK_ARG(k >= 0, "negative dimension");
   B2S_CHECK_ARG(nrows < 2147483647LL, "nrows >= 2^31-1 is not supported");
-  B2S_CHECK_ARG(pt == B2S_I64 || nnz < 2147483647LL, "int32 indptr cannot address nnz >= 2^31-1");
   B2S_CHECK_ARG(ldx >= k && ldy >= k, "leading dimensions (%lld, %lld) smaller than k = %lld", (long long)ldx,
                 (long long)ldy, (long long)k);
   if (nrows == 0 || k == 0) return B2S_OK;

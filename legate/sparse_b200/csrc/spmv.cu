@@ -88,15 +88,12 @@ __global__ void spmv_plan_shape_kernel(const P* __restrict__ indptr, int64_t nti
 static int check_common(int vt, int it, int pt, int64_t nrows, int64_t ncols, int64_t nnz, const void* indptr,
                         const void* indices, const void* vals, const void* x, const void* y) {
   B2S_CHECK_ARG(vt == B2S_F32 || vt == B2S_F64, "bad value type code %d", vt);
-  B2S_CHECK_ARG(it == B2S_I32 || it == B2S_I64, "bad index type code %d", it);
-  B2S_CHECK_ARG(pt == B2S_I32 || pt == B2S_I64, "bad indptr type code %d", pt);
-  B2S_CHECK_ARG(nrows >= 0 && ncols >= 0 && nnz >= 0, "negative dimension");
+  if (int rc = check_csr(it, pt, nrows, ncols, nnz)) return rc;
   B2S_CHECK_ARG(nrows < 2147483647LL, "nrows >= 2^31-1 is not supported");
   B2S_CHECK_ARG(indptr != nullptr, "indptr is NULL");
   B2S_CHECK_ARG(nnz == 0 || (indices != nullptr && vals != nullptr), "indices/vals NULL with nnz > 0");
   B2S_CHECK_ARG(ncols == 0 || nnz == 0 || x != nullptr, "x is NULL");
   B2S_CHECK_ARG(nrows == 0 || y != nullptr, "y is NULL");
-  B2S_CHECK_ARG(pt == B2S_I64 || nnz < 2147483647LL, "int32 indptr cannot address nnz >= 2^31-1");
   return B2S_OK;
 }
 
@@ -579,7 +576,11 @@ static int plan_create_impl(int vt, int it, int pt, int64_t nrows, int64_t ncols
                             const void* indices, void* plan_buf, void* stream, void** plan_out, int flags) {
   B2S_CHECK_ARG(plan_out != nullptr, "plan_out is NULL");
   *plan_out = nullptr;
-  if (int rc = check_common(vt, it, pt, nrows, ncols, nnz, indptr, indices, indices, plan_out, plan_out)) return rc;
+  B2S_CHECK_ARG(vt == B2S_F32 || vt == B2S_F64, "bad value type code %d", vt);
+  if (int rc = check_csr(it, pt, nrows, ncols, nnz)) return rc;
+  B2S_CHECK_ARG(nrows < 2147483647LL, "nrows >= 2^31-1 is not supported");
+  B2S_CHECK_ARG(indptr != nullptr, "indptr is NULL");
+  B2S_CHECK_ARG(nnz == 0 || indices != nullptr, "indices NULL with nnz > 0");
   B2S_CHECK_ARG(plan_buf != nullptr && aligned16(plan_buf), "plan buffer must be non-NULL and 16-byte aligned");
   cudaStream_t st = (cudaStream_t)stream;
   PlanEntry* dev = (PlanEntry*)plan_buf;

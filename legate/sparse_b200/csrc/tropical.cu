@@ -179,12 +179,10 @@ extern "C" {
 int b2s_tropical_spmv_csr(int it, int pt, int64_t nrows, int64_t ncols, int64_t nnz, int64_t nfields,
                           const void* indptr, const void* indices, const void* x, int64_t ldx, void* y, int64_t ldy,
                           void* stream) {
-  B2S_CHECK_ARG(it == B2S_I32 || it == B2S_I64, "bad index type code %d", it);
-  B2S_CHECK_ARG(pt == B2S_I32 || pt == B2S_I64, "bad indptr type code %d", pt);
-  B2S_CHECK_ARG(nrows >= 0 && ncols >= 0 && nnz >= 0 && nfields >= 0, "negative dimension");
+  if (int rc = check_csr(it, pt, nrows, ncols, nnz)) return rc;
+  B2S_CHECK_ARG(nfields >= 0, "negative dimension");
   B2S_CHECK_ARG(nrows < 2147483647LL, "nrows >= 2^31-1 is not supported");
   B2S_CHECK_ARG(nfields < 2147483647LL, "nfields >= 2^31-1 is not supported");
-  B2S_CHECK_ARG(pt == B2S_I64 || nnz < 2147483647LL, "int32 indptr cannot address nnz >= 2^31-1");
   B2S_CHECK_ARG(ldx >= nfields && ldy >= nfields, "leading dimensions (%lld, %lld) smaller than nfields = %lld",
                 (long long)ldx, (long long)ldy, (long long)nfields);
   if (nrows == 0 || nfields == 0) return B2S_OK;
@@ -192,12 +190,9 @@ int b2s_tropical_spmv_csr(int it, int pt, int64_t nrows, int64_t ncols, int64_t 
   B2S_CHECK_ARG(y != nullptr, "y is NULL");
   B2S_CHECK_ARG(nnz == 0 || ncols > 0, "nnz > 0 in a matrix with no columns");
   B2S_CHECK_ARG(nnz == 0 || (indices != nullptr && x != nullptr), "indices/x NULL with nnz > 0");
-  if (x != nullptr && ncols > 0) {
-    // byte ranges [lo, hi) each operand spans; the kernel reads x rows while other rows of y are written
-    const uintptr_t xlo = (uintptr_t)x, xhi = xlo + (uintptr_t)(((ncols - 1) * ldx + nfields) * 8);
-    const uintptr_t ylo = (uintptr_t)y, yhi = ylo + (uintptr_t)(((nrows - 1) * ldy + nfields) * 8);
-    B2S_CHECK_ARG(xhi <= ylo || yhi <= xlo, "x and y overlap");
-  }
+  // the kernel reads x rows while other rows of y are written
+  B2S_CHECK_ARG(ncols == 0 || disjoint(x, ((ncols - 1) * ldx + nfields) * 8, y, ((nrows - 1) * ldy + nfields) * 8),
+                "x and y overlap");
   cudaStream_t st = (cudaStream_t)stream;
   const int nf = (int)nfields;
   const bool v2 = nf == 2 && ldx % 2 == 0 && aligned16(x);

@@ -262,8 +262,7 @@ int b2s_cg_update_xr(int vt, int64_t n, void* x, void* r, const void* p, const v
 int b2s_csr_diagonal(int vt, int it, int pt, int64_t nrows, const void* indptr, const void* indices,
                      const void* vals, void* diag_out, void* stream) {
   B2S_CHECK_ARG(vt == B2S_F32 || vt == B2S_F64, "bad value type code %d", vt);
-  B2S_CHECK_ARG((it == B2S_I32 || it == B2S_I64) && (pt == B2S_I32 || pt == B2S_I64), "bad index type codes");
-  B2S_CHECK_ARG(nrows >= 0, "negative dimension");
+  if (int rc = check_csr(it, pt, nrows, 0, 0)) return rc;
   if (nrows == 0) return B2S_OK;
   B2S_CHECK_ARG(indptr && diag_out, "NULL pointer");
   cudaStream_t st = (cudaStream_t)stream;
