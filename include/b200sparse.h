@@ -457,6 +457,44 @@ int         b2s_csr_lookup(int vt, int it, int pt, int64_t nrows, int64_t ncols,
                            const void* indices, const void* vals, int64_t k, const int64_t* ri, const int64_t* ci,
                            void* out, void* bad, void* stream);
 
+/* ---- assembly from blocks: kron, kronsum, bmat, hstack, vstack, block_diag ------------------------------------------
+ * Nothing is summed, sorted or pruned, so the caller knows nnz_out without reading the device, every output row
+ * pointer has a closed form, and neither entry point syncs, allocates or reads anything back.  Operand row pointers
+ * start at 0.  out_indptr is int64 (nrows_out + 1); out_indices has width ot (B2S_I32 only for ncols_out <= 2^31).  The
+ * outputs must not overlap the inputs or each other.
+ *
+ * b2s_csr_kron: C = kron(A, B), A (am x an), B (bm x bn), values vt (B2S_F32 / B2S_F64) on both.  Output row
+ * i * bm + r holds, for each stored entry (j, a) of row i of A in stored order, row r of B in stored order: columns
+ * j * bn + c, values a * b (one IEEE multiply).  nnz_out = a_nnz * b_nnz; each operand is read in its own index and
+ * indptr widths.  Two launches (row pointers, emit). */
+int         b2s_csr_kron(int vt, int ot, int a_it, int a_pt, int64_t a_nrows, int64_t a_ncols, int64_t a_nnz,
+                         const void* a_indptr, const void* a_indices, const void* a_vals, int b_it, int b_pt,
+                         int64_t b_nrows, int64_t b_ncols, int64_t b_nnz, const void* b_indptr, const void* b_indices,
+                         const void* b_vals, int64_t* out_indptr, void* out_indices, void* out_vals, void* stream);
+
+/* b2s_csr_blocks: bmat of a grid of CSR blocks, given as one descriptor per block with stored entries (None and empty
+ * blocks have none).  Output row row_off + r of a block row is the concatenation, over its descriptors in order, of row
+ * r of each block with columns shifted by col_off.  Descriptors are ordered by block row, the blocks of one block row
+ * share row_off and nrows and go left to right without overlapping columns, block rows go top to bottom without
+ * overlapping rows; every block lies inside nrows_out x ncols_out and the block nnz add up to nnz_out.  Values are
+ * moved, not combined: vw = 4, 8 or 16 bytes.  The table is checked on the host and uploaded into `scratch`
+ * (b2s_csr_blocks_scratch_bytes(ndesc) bytes, device); the number of launches (one upload, row pointers, emit) does
+ * not depend on the number of blocks. */
+typedef struct {
+  const void* indptr;   /* nrows + 1 entries of width pt */
+  const void* indices;  /* nnz entries of width it */
+  const void* vals;     /* nnz values of width vw */
+  int32_t it, pt;       /* B2S_I32 / B2S_I64 */
+  int64_t nrows, ncols, nnz;
+  int64_t row_block;    /* index of the block row */
+  int64_t row_off;      /* output row of the block's row 0 */
+  int64_t col_off;      /* output column of the block's column 0 */
+} b2s_block_desc;
+int64_t     b2s_csr_blocks_scratch_bytes(int64_t ndesc);
+int         b2s_csr_blocks(int vw, int ot, int64_t nrows_out, int64_t ncols_out, int64_t nnz_out, int64_t ndesc,
+                           const b2s_block_desc* desc, int64_t* out_indptr, void* out_indices, void* out_vals,
+                           void* scratch, void* stream);
+
 /* ---- multi-GPU: NCCL communicator owned by the library (SURVEY 8b) -----------------------------------------
  * For hosts without torch.distributed (and for multi-node runs): the library binds NCCL at run time (dlopen of
  * libnccl.so.2, the one already in the process if any) and owns the communicator.  The reference uses NCCL

@@ -8,7 +8,9 @@ hand-written sm_90a kernels in libb200sparse.so (no cuSPARSE, no Legion, no CPU 
 from . import _lib  # noqa: F401  (loads libb200sparse.so; raises if it is missing)
 from .coo import coo_array  # noqa: F401
 from .csr import csr_array, csr_matrix, spgemm_csr_csr_csr  # noqa: F401
-from .module import diags, eye, identity, is_sparse_matrix  # noqa: F401
+from .module import (  # noqa: F401
+    block_diag, bmat, diags, eye, hstack, identity, is_sparse_matrix, kron, kronsum, vstack,
+)
 from .runtime import runtime  # noqa: F401
 from . import io, linalg  # noqa: F401
 

@@ -9,6 +9,8 @@ from __future__ import annotations
 import ctypes
 import os
 
+import numpy as np
+
 from . import _build
 
 c_i32 = ctypes.c_int
@@ -99,6 +101,10 @@ SIGNATURES = {
                                c_i64, c_i64, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp]),
     "b2s_csr_lookup": (c_i32, [c_i32, c_i32, c_i32, c_i64, c_i64, c_i64, c_vp, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp,
                                c_vp, c_vp]),
+    "b2s_csr_kron": (c_i32, [c_i32, c_i32, c_i32, c_i32, c_i64, c_i64, c_i64, c_vp, c_vp, c_vp, c_i32, c_i32, c_i64,
+                             c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "b2s_csr_blocks_scratch_bytes": (c_i64, [c_i64]),
+    "b2s_csr_blocks": (c_i32, [c_i32, c_i32, c_i64, c_i64, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "b2s_comm_nccl_version": (c_i32, []),
     "b2s_comm_unique_id": (c_i32, [c_vp]),
     "b2s_comm_init": (c_i32, [c_i32, c_i32, c_vp, ctypes.POINTER(c_vp)]),
@@ -134,6 +140,13 @@ class FuseDesc(ctypes.Structure):
         ("expect", ctypes.c_uint64),
         ("error", c_vp),
     ]
+
+
+# b2s_block_desc of include/b200sparse.h (one block of b2s_csr_blocks), as a numpy record so a table of many blocks
+# is filled column by column
+BLOCK_DESC = np.dtype([("indptr", np.uint64), ("indices", np.uint64), ("vals", np.uint64), ("it", np.int32),
+                       ("pt", np.int32), ("nrows", np.int64), ("ncols", np.int64), ("nnz", np.int64),
+                       ("row_block", np.int64), ("row_off", np.int64), ("col_off", np.int64)])
 
 
 class B200SparseError(RuntimeError):

@@ -9,6 +9,7 @@ from __future__ import annotations
 
 import ctypes
 
+import numpy as np
 import torch
 
 from . import _lib
@@ -554,6 +555,56 @@ def csr_lookup(indptr, indices, data, shape, ri, ci):
                                 ptr(bad), _stream()),
                "b2s_csr_lookup")
     return out, bad
+
+
+def csr_kron(a_indptr, a_indices, a_data, a_shape, b_indptr, b_indices, b_data, b_shape, out_index_dtype):
+    """kron(A, B) through b2s_csr_kron: (indptr int64, indices of out_index_dtype, data).  Each operand is read in its
+    own index widths; A and B share a value dtype (float32 / float64).  Nothing syncs."""
+    _chk_dev(a_indptr, a_indices, a_data, b_indptr, b_indices, b_data)
+    assert a_data.dtype == b_data.dtype
+    (am, an), (bm, bn) = a_shape, b_shape
+    a_indices, a_data, b_indices, b_data = (t.contiguous() for t in (a_indices, a_data, b_indices, b_data))
+    annz, bnnz = int(a_data.shape[0]), int(b_data.shape[0])
+    dev = a_data.device
+    out_ptr = torch.empty(am * bm + 1, dtype=torch.int64, device=dev)
+    out_idx = torch.empty(annz * bnnz, dtype=out_index_dtype, device=dev)
+    out_val = torch.empty(annz * bnnz, dtype=a_data.dtype, device=dev)
+    _lib.check(L.b2s_csr_kron(vt_code(a_data.dtype), idx_code(out_index_dtype), idx_code(a_indices.dtype),
+                              idx_code(a_indptr.dtype), am, an, annz, ptr(a_indptr), ptr(a_indices), ptr(a_data),
+                              idx_code(b_indices.dtype), idx_code(b_indptr.dtype), bm, bn, bnnz, ptr(b_indptr),
+                              ptr(b_indices), ptr(b_data), ptr(out_ptr), ptr(out_idx), ptr(out_val), _stream()),
+               "b2s_csr_kron")
+    return out_ptr, out_idx, out_val
+
+
+def csr_blocks(blocks, shape, nnz: int, dtype, out_index_dtype):
+    """bmat through b2s_csr_blocks: `blocks` lists (row_block, row_off, col_off, indptr, indices, data, (m, n)) for the
+    blocks with stored entries, in block-row order and left to right; their data share `dtype`, of 4, 8 or 16 bytes.
+    Returns (indptr int64, indices of out_index_dtype, data).  Uploads the block table; nothing syncs."""
+    nrows, ncols = shape
+    dev = runtime.device
+    table = np.zeros(len(blocks), dtype=_lib.BLOCK_DESC)
+    if blocks:
+        rb, ro, co, ip, ix, dv, shp = zip(*blocks)
+        _chk_dev(*ip, *ix, *dv)
+        ix = [t.contiguous() for t in ix]
+        dv = [t.contiguous() for t in dv]
+        table["indptr"] = [t.data_ptr() for t in ip]
+        table["indices"] = [t.data_ptr() for t in ix]
+        table["vals"] = [t.data_ptr() for t in dv]
+        table["it"] = [idx_code(t.dtype) for t in ix]
+        table["pt"] = [idx_code(t.dtype) for t in ip]
+        table["nrows"], table["ncols"] = zip(*shp)
+        table["nnz"] = [t.shape[0] for t in dv]
+        table["row_block"], table["row_off"], table["col_off"] = rb, ro, co
+    out_ptr = torch.empty(nrows + 1, dtype=torch.int64, device=dev)
+    out_idx = torch.empty(nnz, dtype=out_index_dtype, device=dev)
+    out_val = torch.empty(nnz, dtype=dtype, device=dev)
+    scratch = torch.empty(int(L.b2s_csr_blocks_scratch_bytes(len(blocks))), dtype=torch.uint8, device=dev)
+    _lib.check(L.b2s_csr_blocks(out_val.element_size(), idx_code(out_index_dtype), nrows, ncols, nnz, len(blocks),
+                                table.ctypes.data, ptr(out_ptr), ptr(out_idx), ptr(out_val), ptr(scratch), _stream()),
+               "b2s_csr_blocks")
+    return out_ptr, out_idx, out_val
 
 
 def spgemm_row_work(a_indptr, a_indices, b_indptr) -> torch.Tensor:

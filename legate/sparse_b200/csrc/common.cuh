@@ -66,6 +66,19 @@ inline int with_index_types(int it, int pt, F&& f) {
   return with_index_type(it, [&](auto i) { return with_index_type(pt, [&](auto p) { return f(i, p); }); });
 }
 
+// Values that are only moved, never combined (selection, assembly from blocks), by their width in bytes: 4, 8 or 16
+// (fp32, fp64, complex64, complex128 -- or any other element type of that width).  f(W{}) with W uint32_t, uint64_t or
+// Val16.
+struct alignas(16) Val16 { unsigned long long lo, hi; };
+template <typename F>
+inline int with_value_width(int vw, F&& f) {
+  if (vw == 4) return f(uint32_t{});
+  if (vw == 8) return f(uint64_t{});
+  if (vw == 16) return f(Val16{});
+  set_error("bad value width %d", vw);
+  return B2S_EINVAL;
+}
+
 struct DeviceProps {
   int sm_count;
   int max_smem_optin;
@@ -87,6 +100,10 @@ __device__ __forceinline__ double* ws_partials(void* ws) { return reinterpret_ca
 // ---- streaming (read-once) loads: evict-first so the matrix stream does not push the
 // dense x vector out of L2; x itself goes through the default/read-only path. --------------
 template <typename T> __device__ __forceinline__ T ld_stream(const T* p) { return __ldcs(p); }
+template <> __device__ __forceinline__ Val16 ld_stream<Val16>(const Val16* p) {
+  const ulonglong2 v = __ldcs(reinterpret_cast<const ulonglong2*>(p));
+  return Val16{v.x, v.y};
+}
 
 // 4 consecutive elements with 16-byte loads. p must be 16-byte aligned.
 __device__ __forceinline__ void ld_stream4(const int32_t* p, int32_t (&o)[4]) {

@@ -33,8 +33,6 @@ constexpr int IX_WARP_MAX = 4096;    // longest source row one warp handles; lon
 // counters at the head of the scratch buffer
 enum { IX_BAD = 0, IX_NMED = 1, IX_NLONG = 2 };
 
-struct alignas(16) Val16 { unsigned long long lo, hi; };
-
 // evict-first load of one value or index of any width the selection moves
 template <typename T> __device__ __forceinline__ T ix_ld(const T* p) { return __ldcs(p); }
 template <> __device__ __forceinline__ Val16 ix_ld<Val16>(const Val16* p) {
@@ -298,15 +296,6 @@ static IxScratch ix_layout(int64_t nout) {
   L.off_sums = o;     o += up(cv_scan_sums_bytes(nout + 1));
   L.total = o;
   return L;
-}
-
-template <typename F>
-inline int with_value_width(int vw, F&& f) {
-  if (vw == 4) return f(uint32_t{});
-  if (vw == 8) return f(uint64_t{});
-  if (vw == 16) return f(Val16{});
-  set_error("bad value width %d", vw);
-  return B2S_EINVAL;
 }
 
 struct SelectArgs {

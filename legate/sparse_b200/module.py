@@ -1,16 +1,30 @@
-"""Construction helpers on the path of the examples: `diags`, `eye`, `identity`, `is_sparse_matrix`.
+"""Construction: `diags`, `eye`, `identity`, `is_sparse_matrix`, and assembly from blocks: `kron`, `kronsum`, `bmat`,
+`hstack`, `vstack`, `block_diag`.
 
-The reference builds these with cuNumeric ops + DIA->CSC conversion (sparse/module.py:96-246,
-sparse/dia.py:175-249: entries equal to zero are dropped by the `data != 0` mask, dia.py:236).
-They are matrix assembly, not the hot path: assembled on the host (vectorised numpy, no scipy
-dependency in the arithmetic) and uploaded as a `csr_array`.
+`diags`, `eye` and `identity` follow the reference (sparse/module.py:96-246, sparse/dia.py:175-249: entries equal to
+zero are dropped by the `data != 0` mask, dia.py:236).  They are small assembly, not the hot path: built on the host
+(vectorised numpy, no scipy dependency in the arithmetic) and uploaded as a `csr_array`.
+
+The block functions run on the device (csrc/construct.cu, DESIGN section 3.13): shapes, dtypes and the block table are
+worked out on the host from the operands' shapes alone, and two kernels write the result without reading anything back.
+They keep every stored entry -- stored order, explicit zeros, repeated columns -- and sum nothing, except `kronsum`,
+which adds its two Kronecker products with the sparse add (a sum that cancels to zero stays stored).  Unlike scipy,
+which returns BSR or COO by default, they return a `csr_array` for `format=None` and `"csr"`, and `result.tocoo()` for
+`"coo"`; this library has no BSR type and no COO compute path, and other formats raise NotImplementedError.
 """
 from __future__ import annotations
 
-import numpy as np
+import numbers
+from itertools import accumulate
 
+import numpy as np
+import scipy.sparse
+import torch
+
+from . import _ops
 from .coo import coo_array
-from .csr import csr_array
+from .csr import _csr_binop, _index_dtype, _indptr_dtype, csr_array
+from .runtime import SUPPORTED_VALUE_DTYPES, runtime, to_host, torch_dtype
 
 
 def is_sparse_matrix(o) -> bool:
@@ -135,3 +149,208 @@ def eye(m, n=None, k=0, dtype=np.float64, format=None):
 
 def identity(n, dtype=np.float64, format=None):
     return eye(n, n, dtype=dtype, format=format)
+
+
+# ---- assembly from blocks (csrc/construct.cu) ---------------------------------------------------------------------------
+_INT64_MAX = 2**63 - 1
+
+
+def _as_csr(x) -> csr_array:
+    """An operand as a csr_array: a csr_array as it is; a coo_array, a scipy sparse matrix or what `diags` returns
+    through its CSR; a dense numpy array or torch tensor through `csr_array(dense)`, which drops zeros (a 1-D array is one
+    row, as scipy reads it)."""
+    if isinstance(x, csr_array):
+        return x
+    if isinstance(x, coo_array):
+        return x.tocsr()
+    if scipy.sparse.issparse(x):
+        return csr_array(x)
+    if isinstance(x, torch.Tensor):
+        x = to_host(x)
+    if not isinstance(x, np.ndarray) and hasattr(x, "tocsr"):
+        return _as_csr(x.tocsr())
+    a = np.atleast_2d(np.asarray(x))
+    if a.ndim != 2:
+        raise NotImplementedError(f"a {a.ndim}-D operand cannot be a block")
+    return csr_array(a)
+
+
+def _is_csr(x) -> bool:
+    """scipy's test for its CSR stacking path: a sparse matrix in CSR format"""
+    return isinstance(x, csr_array) or (scipy.sparse.issparse(x) and x.format == "csr")
+
+
+def _check_result(shape, nnz, format, what):
+    """The host checks every assembly makes before it allocates: the result fits int64 indices, and the format is one
+    this library returns."""
+    if max(shape[0], shape[1], nnz) >= _INT64_MAX:
+        raise ValueError(f"{what}: a {shape[0]} x {shape[1]} result with {nnz} stored entries does not fit in int64")
+    if format not in (None, "csr", "coo"):
+        raise NotImplementedError(f"{what}(format={format!r}): only 'csr' (the default) and 'coo' results are built")
+
+
+def _finish(C: csr_array, format):
+    return C.tocoo() if format == "coo" else C
+
+
+def kron(A, B, format=None):
+    """Kronecker product of A (m x n) and B (p x q), scipy.sparse.kron on the device (reference sparse/module.py).
+
+    Output row i * p + r holds, for each stored entry (j, a) of row i of A in stored order, row r of B in stored order,
+    with columns j * q + c and values a * b.  Stored order, explicit zeros and repeated columns are kept, so canonical
+    operands give a canonical result, equal to scipy's bit for bit.  The dtype is np.result_type of the operands,
+    float32 or float64 (others raise NotImplementedError); only an operand of another dtype is cast.  Returns a
+    csr_array (format None / "csr") or its tocoo() ("coo")."""
+    A, B = _as_csr(A), _as_csr(B)
+    shape = (A.shape[0] * B.shape[0], A.shape[1] * B.shape[1])
+    nnz = A.nnz * B.nnz
+    _check_result(shape, nnz, format, "kron")
+    dtype = np.result_type(A.dtype, B.dtype)
+    if dtype not in SUPPORTED_VALUE_DTYPES:
+        raise NotImplementedError(f"kron for dtype {dtype} is not implemented (float32/float64 kernels only)")
+    runtime.require_cuda("kron")
+    A, B = A.astype(dtype, copy=False), B.astype(dtype, copy=False)
+    ptr, idx, val = _ops.csr_kron(A._indptr, A._indices, A._data, A.shape, B._indptr, B._indices, B._data, B.shape,
+                                  _index_dtype(shape[1] - 1))
+    return _finish(csr_array._from_parts(ptr.to(_indptr_dtype(nnz)), idx, val, shape), format)
+
+
+def _identity(n: int, dtype) -> csr_array:
+    ar = torch.arange(n + 1, dtype=torch.int64, device=runtime.device)
+    return csr_array._from_parts(ar.to(_indptr_dtype(n)), ar[:n].to(_index_dtype(n - 1)),
+                                 torch.ones(n, dtype=torch_dtype(dtype), device=runtime.device), (n, n))
+
+
+def kronsum(A, B, format=None):
+    """Kronecker sum of square A (m x m) and B (n x n): kron(I_n, A) + kron(B, I_m), scipy's definition.  The two
+    products come from `kron` and are added by the sparse add (csrc/elementwise.cu), which keeps entries that cancel to
+    zero where scipy drops them.  Raises ValueError for a non-square operand, as scipy does."""
+    A, B = _as_csr(A), _as_csr(B)
+    if A.shape[0] != A.shape[1]:
+        raise ValueError("A is not square")
+    if B.shape[0] != B.shape[1]:
+        raise ValueError("B is not square")
+    m, n = A.shape[0], B.shape[0]
+    _check_result((m * n, m * n), n * A.nnz + m * B.nnz, format, "kronsum")
+    dtype = np.result_type(A.dtype, B.dtype)
+    if dtype not in SUPPORTED_VALUE_DTYPES:
+        raise NotImplementedError(f"kronsum for dtype {dtype} is not implemented (float32/float64 kernels only)")
+    runtime.require_cuda("kronsum")
+    C = _csr_binop(kron(_identity(n, dtype), A), kron(B, _identity(m, dtype)), "add")
+    return _finish(C, format)
+
+
+def _assemble(placed, shape, dtype, format, what):
+    """The csr_array of the blocks `placed` = [(block row, row offset, column offset, csr_array)], in block-row order
+    and left to right within a block row, through b2s_csr_blocks."""
+    nnz = sum(A.nnz for _, _, _, A in placed)
+    _check_result(shape, nnz, format, what)
+    dtype = np.dtype(dtype)
+    if dtype.itemsize not in (4, 8, 16) or dtype.kind not in "fciu":
+        raise NotImplementedError(f"{what} for dtype {dtype} is not implemented (4-, 8- or 16-byte values)")
+    runtime.require_cuda(what)
+    tdt = torch_dtype(dtype)
+    blocks = [(I, ro, co, A._indptr, A._indices, A._data if A._data.dtype == tdt else A._data.to(tdt), A.shape)
+              for I, ro, co, A in placed if A.nnz]
+    ptr, idx, val = _ops.csr_blocks(blocks, shape, nnz, tdt, _index_dtype(shape[1] - 1))
+    return _finish(csr_array._from_parts(ptr.to(_indptr_dtype(nnz)), idx, val, shape), format)
+
+
+def _result_dtype(mats, dtype):
+    if dtype is not None:
+        return np.dtype(dtype)
+    return np.result_type(*[A.dtype for A in mats]) if mats else np.dtype(np.float64)
+
+
+def bmat(blocks, format=None, dtype=None):
+    """A sparse matrix from a 2-D grid of blocks (None: an all-zero block), scipy.sparse.bmat on the device.
+
+    Output row r of block row I is the concatenation, over the block columns in order, of row r of each block, its
+    columns shifted by the width of the blocks to its left.  Entries keep their stored order; nothing is summed or
+    pruned.  Shapes are checked as scipy 1.18.1 checks them: when every block is a CSR matrix and format is None or
+    "csr", scipy stacks each block row horizontally and the rows vertically, so the blocks of a row must share a height
+    and the rows a total width; otherwise every block row has one height and every block column one width, a block
+    with no rows or columns leaving its row's or column's size open.  The dtype is np.result_type of the blocks (or
+    `dtype`), of 4, 8 or 16 bytes; only blocks of another dtype are cast.  Returns a csr_array (format None / "csr")
+    or its tocoo() ("coo")."""
+    grid = np.asarray(blocks, dtype="object")
+    if grid.ndim != 2:
+        raise ValueError("blocks must be 2-D, and some must be sparse")
+    M, N = grid.shape
+    placed = []
+    if format in (None, "csr") and all(_is_csr(b) for b in grid.flat):
+        if N == 0:
+            raise IndexError(f"index 0 is out of bounds for axis 1 with size {N}")
+        if M == 0:
+            raise ValueError("need at least one array to concatenate")
+        rows = [[_as_csr(b) for b in grid[I]] for I in range(M)]
+        for row in rows:
+            heights = {A.shape[0] for A in row}
+            if len(heights) > 1:
+                raise ValueError(f"Mismatching dimensions along axis 0: {heights}")
+        widths = [sum(A.shape[1] for A in row) for row in rows]
+        if any(w != widths[0] for w in widths):
+            raise ValueError("incompatible dimensions for axis 1")
+        r = 0
+        for I, row in enumerate(rows):
+            c = 0
+            for A in row:
+                placed.append((I, r, c, A))
+                c += A.shape[1]
+            r += row[0].shape[0]
+        shape = (r, widths[0])
+    else:
+        brow, bcol = [0] * M, [0] * N
+        mats = {}
+        for i in range(M):
+            for j in range(N):
+                if grid[i, j] is None:
+                    continue
+                A = mats[i, j] = _as_csr(grid[i, j])
+                if brow[i] == 0:
+                    brow[i] = A.shape[0]
+                elif brow[i] != A.shape[0]:
+                    raise ValueError(f"blocks[{i},:] has incompatible row dimensions. Got blocks[{i},{j}].shape[0] == "
+                                     f"{A.shape[0]}, expected {brow[i]}.")
+                if bcol[j] == 0:
+                    bcol[j] = A.shape[1]
+                elif bcol[j] != A.shape[1]:
+                    raise ValueError(f"blocks[:,{j}] has incompatible column dimensions. Got blocks[{i},{j}].shape[1] "
+                                     f"== {A.shape[1]}, expected {bcol[j]}.")
+        roff, coff = [0, *accumulate(brow)], [0, *accumulate(bcol)]
+        placed = [(i, roff[i], coff[j], A) for (i, j), A in mats.items()]
+        shape = (roff[-1], coff[-1])
+    return _assemble(placed, shape, _result_dtype([A for *_, A in placed], dtype), format, "bmat")
+
+
+def hstack(blocks, format=None, dtype=None):
+    """Blocks side by side: bmat([blocks]), as scipy.sparse.hstack."""
+    return bmat([np.asarray(blocks, dtype="object")], format=format, dtype=dtype)
+
+
+def vstack(blocks, format=None, dtype=None):
+    """Blocks one above the other: bmat([[b] for b in blocks]), as scipy.sparse.vstack."""
+    return bmat([[b] for b in np.asarray(blocks, dtype="object")], format=format, dtype=dtype)
+
+
+def block_diag(mats, format=None, dtype=None):
+    """A block-diagonal matrix of `mats`, scipy.sparse.block_diag on the device: blocks as bmat takes them, and scalars
+    (and lists) as dense arrays of at least two dimensions, so a scalar is a 1 x 1 block.  Dense blocks drop their
+    zeros (scipy keeps the zeros of dense ndarray blocks as stored entries)."""
+    placed = []
+    r = c = 0
+    for k, a in enumerate(mats):
+        if isinstance(a, (list, numbers.Number)):
+            A = csr_array(np.atleast_2d(a))
+        elif isinstance(a, (np.ndarray, torch.Tensor)):
+            if a.ndim != 2:  # scipy unpacks a dense block's shape into (rows, columns)
+                raise ValueError(f"a dense block must be 2-D, got shape {tuple(a.shape)}")
+            A = _as_csr(a)
+        else:
+            A = _as_csr(a)
+        placed.append((k, r, c, A))
+        r += A.shape[0]
+        c += A.shape[1]
+    if not placed:
+        raise ValueError("need at least one array to concatenate")
+    return _assemble(placed, (r, c), _result_dtype([A for *_, A in placed], dtype), format, "block_diag")

@@ -3,17 +3,23 @@ legate.sparse_b200, so a script written against the reference package runs uncha
 (CSR construction, SpMV, SpGEMM, CG).  Everything lives in legate/sparse_b200; nothing is implemented here."""
 from legate.sparse_b200 import *  # noqa: F401,F403
 from legate.sparse_b200 import (  # noqa: F401
+    block_diag,
+    bmat,
     coo_array,
     coo_matrix,
     csr_array,
     csr_matrix,
     diags,
     eye,
+    hstack,
     identity,
     io,
     is_sparse_matrix,
+    kron,
+    kronsum,
     linalg,
     runtime,
+    vstack,
 )
 
 
