@@ -495,6 +495,24 @@ int         b2s_csr_blocks(int vw, int ot, int64_t nrows_out, int64_t ncols_out,
                            const b2s_block_desc* desc, int64_t* out_indptr, void* out_indices, void* out_vals,
                            void* scratch, void* stream);
 
+/* ---- CSC products: y = A x and Y = A X for a CSC matrix A (nrows x ncols) ---------------------------------------
+ * Replace CSCSpMV::gpu_variant (src/sparse/array/csc/spmv.cu) and CSCSpMM::gpu_variant (src/sparse/array/csc/spmm.cu),
+ * built by sparse/csc.py.  indptr has ncols + 1 entries and `indices` are row ids: the arrays of the CSR matrix of A's
+ * transpose, so the operand is checked as that CSR operand (Conventions, with nrows and ncols swapped).  Rows within a
+ * column may be unsorted or repeated; repeated entries are summed.  x has ncols values and y nrows; X is (ncols x k) and
+ * Y (nrows x k), row-major with row strides ldx, ldy >= k.  y and Y are written in full (zeroed on the stream, then
+ * every stored entry adds its product with an atomic), and must not overlap any input.
+ * Determinism: the atomics land in an unspecified order, so a row that receives three or more terms may differ in the
+ * last bits between calls; integer-valued data (every partial sum exactly representable) gives an exact result.  fp32
+ * atomics flush subnormal products to zero.  The CSR product of the transpose is the deterministic alternative.
+ * No host sync, no allocation: capturable in a CUDA graph. */
+int         b2s_spmv_csc(int vt, int it, int pt, int64_t nrows, int64_t ncols, int64_t nnz,
+                         const void* indptr, const void* indices, const void* vals,
+                         const void* x, void* y, void* stream);
+int         b2s_spmm_csc(int vt, int it, int pt, int64_t nrows, int64_t ncols, int64_t nnz, int64_t k,
+                         const void* indptr, const void* indices, const void* vals,
+                         const void* X, int64_t ldx, void* Y, int64_t ldy, void* stream);
+
 /* ---- multi-GPU: NCCL communicator owned by the library (SURVEY 8b) -----------------------------------------
  * For hosts without torch.distributed (and for multi-node runs): the library binds NCCL at run time (dlopen of
  * libnccl.so.2, the one already in the process if any) and owns the communicator.  The reference uses NCCL

@@ -7,6 +7,7 @@ hand-written sm_90a kernels in libb200sparse.so (no cuSPARSE, no Legion, no CPU 
 """
 from . import _lib  # noqa: F401  (loads libb200sparse.so; raises if it is missing)
 from .coo import coo_array  # noqa: F401
+from .csc import csc_array, csc_matrix  # noqa: F401
 from .csr import csr_array, csr_matrix, spgemm_csr_csr_csr  # noqa: F401
 from .module import (  # noqa: F401
     block_diag, bmat, diags, eye, hstack, identity, is_sparse_matrix, kron, kronsum, vstack,

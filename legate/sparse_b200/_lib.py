@@ -105,6 +105,9 @@ SIGNATURES = {
                              c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "b2s_csr_blocks_scratch_bytes": (c_i64, [c_i64]),
     "b2s_csr_blocks": (c_i32, [c_i32, c_i32, c_i64, c_i64, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "b2s_spmv_csc": (c_i32, [c_i32, c_i32, c_i32, c_i64, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "b2s_spmm_csc": (c_i32, [c_i32, c_i32, c_i32, c_i64, c_i64, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp,
+                             c_i64, c_vp]),
     "b2s_comm_nccl_version": (c_i32, []),
     "b2s_comm_unique_id": (c_i32, [c_vp]),
     "b2s_comm_init": (c_i32, [c_i32, c_i32, c_vp, ctypes.POINTER(c_vp)]),

@@ -204,6 +204,36 @@ def spmm(indptr, indices, data, X, Y, shape):
     return Y
 
 
+def spmv_csc(indptr, indices, data, x, y, shape):
+    """y = A @ x for a CSC matrix A of `shape` (indptr over columns, indices = rows) through b2s_spmv_csc (replaces task
+    CSC_SPMV, sparse/csc.py:523-553).  y is overwritten; the launch neither syncs nor allocates."""
+    _chk_dev(indptr, indices, data, x, y)
+    nrows, ncols = shape
+    assert x.dtype == data.dtype == y.dtype and x.is_contiguous() and y.is_contiguous()
+    assert x.shape[0] == ncols and y.shape[0] == nrows and indptr.shape[0] == ncols + 1
+    _lib.check(L.b2s_spmv_csc(vt_code(data.dtype), idx_code(indices.dtype), idx_code(indptr.dtype), nrows, ncols,
+                              int(data.shape[0]), ptr(indptr), ptr(indices.contiguous()), ptr(data.contiguous()), ptr(x),
+                              ptr(y), _stream()), "b2s_spmv_csc")
+    return y
+
+
+def spmm_csc(indptr, indices, data, X, Y, shape):
+    """Y = A @ X for a CSC matrix A and row-major dense X (ncols, k), Y (nrows, k) through b2s_spmm_csc (replaces task
+    CSC_SPMM, sparse/csc.py:630-680).  Rows of X / Y may be strided; the k entries of a row must be contiguous."""
+    _chk_dev(indptr, indices, data, X, Y)
+    nrows, ncols = shape
+    assert X.dtype == data.dtype == Y.dtype and X.ndim == 2 and Y.ndim == 2
+    k = X.shape[1]
+    assert X.shape[0] == ncols and tuple(Y.shape) == (nrows, k) and indptr.shape[0] == ncols + 1
+    assert k <= 1 or ((ncols == 0 or X.stride(1) == 1) and (nrows == 0 or Y.stride(1) == 1))
+    ldx = X.stride(0) if X.shape[0] > 1 else max(k, 1)
+    ldy = Y.stride(0) if Y.shape[0] > 1 else max(k, 1)
+    _lib.check(L.b2s_spmm_csc(vt_code(data.dtype), idx_code(indices.dtype), idx_code(indptr.dtype), nrows, ncols,
+                              int(data.shape[0]), k, ptr(indptr), ptr(indices.contiguous()), ptr(data.contiguous()),
+                              ptr(X), ldx, ptr(Y), ldy, _stream()), "b2s_spmm_csc")
+    return Y
+
+
 def spmv_tiles(indptr, indices, data, x, y, shape, plan, tile_lo: int, tile_hi: int):
     """Rows of tiles [tile_lo, tile_hi) of y = A @ x (x must be valid on that chunk's column window)."""
     _chk_dev(indptr, indices, data, x, y)

@@ -129,6 +129,11 @@ class coo_array:
         np.cumsum(counts, out=indptr[1:])  # nnz_to_pos, reference base.py:30-48
         return csr_array((vals, cols, indptr), shape=self.shape)
 
+    def tocsc(self, copy=False):
+        from .csc import csc_array
+
+        return csc_array(self)
+
     def todense(self):
         vals, i, j = self._host()
         out = np.zeros(self.shape, dtype=self.dtype)
@@ -168,4 +173,6 @@ class coo_array:
             return self
         if format == "csr":
             return self.tocsr()
+        if format == "csc":
+            return self.tocsc()
         raise NotImplementedError(f"format {format!r}")

@@ -212,6 +212,12 @@ class csr_array:
     def tocsr(self, copy=False):
         return self.copy() if copy else self
 
+    def tocsc(self, copy=False):
+        """The CSC form: a csc_array holding the CSR transpose (`transpose`), so new arrays whatever `copy` says."""
+        from .csc import csc_array
+
+        return csc_array(self)
+
     def tocoo(self, copy=False):
         from .coo import coo_array
 
@@ -490,6 +496,11 @@ class csr_array:
             assert self.shape[1] == other.shape[0]
             return spgemm_csr_csr_csr(*cast_to_common_type(self, other))
         if is_sparse_matrix(other) or scipy.sparse.issparse(other):
+            from .csc import csc_array
+
+            if isinstance(other, csc_array):
+                # CSR x CSC is SpGEMM with the cached CSR form, not a dense product
+                return self.dot(other.tocsr(), out=out)
             other = np.asarray(other.todense())
             other_originally_sparse = True
         else:

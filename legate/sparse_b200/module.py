@@ -23,12 +23,13 @@ import torch
 
 from . import _ops
 from .coo import coo_array
+from .csc import csc_array
 from .csr import _csr_binop, _index_dtype, _indptr_dtype, csr_array
 from .runtime import SUPPORTED_VALUE_DTYPES, runtime, to_host, torch_dtype
 
 
 def is_sparse_matrix(o) -> bool:
-    return isinstance(o, (csr_array, coo_array))
+    return isinstance(o, (csr_array, csc_array, coo_array))
 
 
 def _dia_to_csr(diagonals, offsets, shape, dtype):
@@ -70,7 +71,7 @@ class _dia_result:
         return self._csr
 
     def tocsc(self, copy=False):
-        return _csc_view(self._csr)
+        return csc_array(self._csr)
 
     def todense(self):
         return self._csr.todense()
@@ -80,25 +81,6 @@ class _dia_result:
     @property
     def T(self):
         return _dia_result(self._csr.T)
-
-
-class _csc_view:
-    """CSC of M represented by the CSR of M^T; `.T` hands that CSR back (reference csc.py:317-324)."""
-
-    def __init__(self, csr_of_m):
-        self._m = csr_of_m
-        self.shape = csr_of_m.shape
-        self.dtype = csr_of_m.dtype
-
-    @property
-    def T(self):
-        return self._m.T
-
-    def tocsr(self, copy=False):
-        return self._m
-
-    def todense(self):
-        return self._m.todense()
 
 
 def diags(diagonals, offsets=0, shape=None, format=None, dtype=None):
@@ -133,7 +115,7 @@ def diags(diagonals, offsets=0, shape=None, format=None, dtype=None):
     if format in (None, "dia"):
         return _dia_result(csr)
     if format == "csc":
-        return _csc_view(csr)
+        return csc_array(csr)
     raise NotImplementedError(f"diags(format={format!r})")
 
 

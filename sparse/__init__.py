@@ -7,6 +7,8 @@ from legate.sparse_b200 import (  # noqa: F401
     bmat,
     coo_array,
     coo_matrix,
+    csc_array,
+    csc_matrix,
     csr_array,
     csr_matrix,
     diags,
