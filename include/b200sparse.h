@@ -513,6 +513,46 @@ int         b2s_spmm_csc(int vt, int it, int pt, int64_t nrows, int64_t ncols, i
                          const void* indptr, const void* indices, const void* vals,
                          const void* X, int64_t ldx, void* Y, int64_t ldy, void* stream);
 
+/* ---- DIA: diagonal-format matrices ------------------------------------------------------------------------------
+ * Built by sparse/dia.py (the reference's dia.py converts to CSC on the host; it has no DIA kernels).  A DIA matrix
+ * (nrows x ncols) holds ndiag diagonals: int64 `offsets[ndiag]` (any order, no repeats) and `data`, ndiag x L values,
+ * contiguous, column-aligned as in scipy: entry (r, r + offsets[d]) is data[d * L + r + offsets[d]], stored when
+ * 0 <= r < nrows and 0 <= r + offsets[d] < min(ncols, L).  Offsets outside that band are allowed and contribute
+ * nothing.  Every DIA entry point rejects with B2S_EINVAL: a vt other than 0 / 1, a negative nrows, ncols, ndiag or L,
+ * and ndiag * L * 8 beyond int64.
+ *
+ * Products: y[r] = sum over d of data[d, r + k_d] * x[r + k_d], and Y[r, :] likewise with rows of X (ncols x k) and Y
+ * (nrows x k), row-major with row strides ldx, ldy >= k.  Each row of y / Y is computed by one thread or lane group,
+ * summing its in-band diagonals in stored order from zero, in the value type: no atomics, so two calls give identical
+ * results, and integer-valued data (every partial sum exactly representable) gives the exact result.  y and Y are
+ * written in full and must not overlap any input.  No host sync, no allocation: capturable in a CUDA graph. */
+int         b2s_spmv_dia(int vt, int64_t nrows, int64_t ncols, int64_t ndiag, int64_t L, const int64_t* offsets,
+                         const void* data, const void* x, void* y, void* stream);
+int         b2s_spmm_dia(int vt, int64_t nrows, int64_t ncols, int64_t ndiag, int64_t L, int64_t k,
+                         const int64_t* offsets, const void* data, const void* X, int64_t ldx, void* Y, int64_t ldy,
+                         void* stream);
+/* Scratch bytes b2s_dia_to_csr and b2s_csr_to_dia need for an nrows x ncols matrix (0 for negative sizes). */
+int64_t     b2s_dia_scratch_bytes(int64_t nrows, int64_t ncols);
+/* DIA -> CSR, keeping the in-band entries with data != 0 (the value type's `!=`: -0.0 is dropped, NaN kept).  `order`
+ * is the permutation of 0..ndiag-1 that sorts `offsets` ascending; each row is emitted in that order, so its columns
+ * come out sorted.  Two calls, each of which checks the CSR result as an operand (Conventions):
+ *  - indices == vals == NULL: writes indptr[nrows + 1] and *nnz_host (syncs the stream); `nnz` is ignored;
+ *  - otherwise, with the indptr of the first call and nnz = *nnz_host: writes indices[nnz] and vals[nnz].
+ * `scratch`: b2s_dia_scratch_bytes(nrows, ncols) bytes. */
+int         b2s_dia_to_csr(int vt, int it, int pt, int64_t nrows, int64_t ncols, int64_t ndiag, int64_t L,
+                           const int64_t* offsets, const int64_t* order, const void* data, int64_t nnz, void* indptr,
+                           void* indices, void* vals, void* scratch, int64_t scratch_bytes, int64_t* nnz_host,
+                           void* stream);
+/* CSR -> DIA for a CSR operand (Conventions) with no repeated (row, column) in a row.  Two calls with one `scratch` of
+ * b2s_dia_scratch_bytes(nrows, ncols) bytes, left untouched in between:
+ *  - data == NULL: finds the diagonals present and writes ndiag_L_host[0] = their number and ndiag_L_host[1] = the
+ *    largest column + 1 (both 0 when nnz = 0); syncs the stream.  `ndiag`, `L`, `offsets` are ignored;
+ *  - otherwise, with those two values as ndiag and L: writes offsets[ndiag], ascending, and data (ndiag x L), zero
+ *    where no entry is stored.  Each entry is written once; no atomics. */
+int         b2s_csr_to_dia(int vt, int it, int pt, int64_t nrows, int64_t ncols, int64_t nnz, const void* indptr,
+                           const void* indices, const void* vals, int64_t ndiag, int64_t L, int64_t* offsets,
+                           void* data, void* scratch, int64_t scratch_bytes, int64_t* ndiag_L_host, void* stream);
+
 /* ---- multi-GPU: NCCL communicator owned by the library (SURVEY 8b) -----------------------------------------
  * For hosts without torch.distributed (and for multi-node runs): the library binds NCCL at run time (dlopen of
  * libnccl.so.2, the one already in the process if any) and owns the communicator.  The reference uses NCCL

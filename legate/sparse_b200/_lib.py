@@ -108,6 +108,13 @@ SIGNATURES = {
     "b2s_spmv_csc": (c_i32, [c_i32, c_i32, c_i32, c_i64, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "b2s_spmm_csc": (c_i32, [c_i32, c_i32, c_i32, c_i64, c_i64, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp,
                              c_i64, c_vp]),
+    "b2s_spmv_dia": (c_i32, [c_i32, c_i64, c_i64, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "b2s_spmm_dia": (c_i32, [c_i32, c_i64, c_i64, c_i64, c_i64, c_i64, c_vp, c_vp, c_vp, c_i64, c_vp, c_i64, c_vp]),
+    "b2s_dia_scratch_bytes": (c_i64, [c_i64, c_i64]),
+    "b2s_dia_to_csr": (c_i32, [c_i32, c_i32, c_i32, c_i64, c_i64, c_i64, c_i64, c_vp, c_vp, c_vp, c_i64, c_vp, c_vp,
+                               c_vp, c_vp, c_i64, c_vp, c_vp]),
+    "b2s_csr_to_dia": (c_i32, [c_i32, c_i32, c_i32, c_i64, c_i64, c_i64, c_vp, c_vp, c_vp, c_i64, c_i64, c_vp, c_vp,
+                               c_vp, c_i64, c_vp, c_vp]),
     "b2s_comm_nccl_version": (c_i32, []),
     "b2s_comm_unique_id": (c_i32, [c_vp]),
     "b2s_comm_init": (c_i32, [c_i32, c_i32, c_vp, ctypes.POINTER(c_vp)]),

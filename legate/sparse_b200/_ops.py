@@ -234,6 +234,84 @@ def spmm_csc(indptr, indices, data, X, Y, shape):
     return Y
 
 
+def spmv_dia(offsets, data, x, y, shape):
+    """y = A @ x for a DIA matrix A of `shape` (int64 device `offsets`, contiguous `data` of ndiag x L) through
+    b2s_spmv_dia.  y is overwritten; the launch neither syncs nor allocates."""
+    _chk_dev(offsets, data, x, y)
+    nrows, ncols = shape
+    assert x.dtype == data.dtype == y.dtype and x.is_contiguous() and y.is_contiguous() and data.is_contiguous()
+    assert offsets.dtype == torch.int64 and data.ndim == 2 and offsets.shape[0] == data.shape[0]
+    assert x.shape[0] == ncols and y.shape[0] == nrows
+    ndiag, Ld = data.shape
+    _lib.check(L.b2s_spmv_dia(vt_code(data.dtype), nrows, ncols, ndiag, Ld, ptr(offsets), ptr(data), ptr(x), ptr(y),
+                              _stream()), "b2s_spmv_dia")
+    return y
+
+
+def spmm_dia(offsets, data, X, Y, shape):
+    """Y = A @ X for a DIA matrix A and row-major dense X (ncols, k), Y (nrows, k) through b2s_spmm_dia.  Rows of X / Y
+    may be strided; the k entries of a row must be contiguous."""
+    _chk_dev(offsets, data, X, Y)
+    nrows, ncols = shape
+    assert X.dtype == data.dtype == Y.dtype and X.ndim == 2 and Y.ndim == 2 and data.is_contiguous()
+    assert offsets.dtype == torch.int64 and data.ndim == 2 and offsets.shape[0] == data.shape[0]
+    k = X.shape[1]
+    assert X.shape[0] == ncols and tuple(Y.shape) == (nrows, k)
+    assert k <= 1 or ((ncols == 0 or X.stride(1) == 1) and (nrows == 0 or Y.stride(1) == 1))
+    ldx = X.stride(0) if X.shape[0] > 1 else max(k, 1)
+    ldy = Y.stride(0) if Y.shape[0] > 1 else max(k, 1)
+    ndiag, Ld = data.shape
+    _lib.check(L.b2s_spmm_dia(vt_code(data.dtype), nrows, ncols, ndiag, Ld, k, ptr(offsets), ptr(data), ptr(X), ldx,
+                              ptr(Y), ldy, _stream()), "b2s_spmm_dia")
+    return Y
+
+
+def dia_to_csr(offsets, order, data, shape, ptr_dtype, idx_dtype):
+    """CSR arrays (indptr, indices, vals) of a DIA matrix through b2s_dia_to_csr: in-band entries with data != 0, each
+    row's columns ascending (`order` sorts `offsets`).  Reads the nnz back to allocate the result."""
+    _chk_dev(offsets, order, data)
+    nrows, ncols = shape
+    ndiag, Ld = data.shape
+    dev = data.device
+    vt, it, pt = vt_code(data.dtype), idx_code(idx_dtype), idx_code(ptr_dtype)
+    indptr = torch.empty(nrows + 1, dtype=ptr_dtype, device=dev)
+    scratch = torch.empty(max(int(L.b2s_dia_scratch_bytes(nrows, ncols)), 1), dtype=torch.uint8, device=dev)
+    nnz = _lib.c_i64(0)
+    args = (vt, it, pt, nrows, ncols, ndiag, Ld, ptr(offsets), ptr(order), ptr(data))
+    _lib.check(L.b2s_dia_to_csr(*args, 0, ptr(indptr), None, None, ptr(scratch), scratch.numel(), ctypes.byref(nnz),
+                                _stream()), "b2s_dia_to_csr")
+    indices = torch.empty(nnz.value, dtype=idx_dtype, device=dev)
+    vals = torch.empty(nnz.value, dtype=data.dtype, device=dev)
+    if nnz.value:
+            _lib.check(L.b2s_dia_to_csr(*args, nnz.value, ptr(indptr), ptr(indices), ptr(vals), None, 0, None, _stream()),
+                   "b2s_dia_to_csr")
+    return indptr, indices, vals
+
+
+def csr_to_dia(indptr, indices, data, shape, allocate):
+    """(offsets, data) of the DIA form of a CSR matrix with no repeated (row, column) through b2s_csr_to_dia.  The
+    diagonal count and L = largest column + 1 are read back and passed to `allocate(ndiag, L)`, which may raise before
+    anything of that size is allocated; it returns nothing."""
+    _chk_dev(indptr, indices, data)
+    nrows, ncols = shape
+    nnz = int(data.shape[0])
+    dev = data.device
+    vt, it, pt = vt_code(data.dtype), idx_code(indices.dtype), idx_code(indptr.dtype)
+    scratch = torch.empty(max(int(L.b2s_dia_scratch_bytes(nrows, ncols)), 1), dtype=torch.uint8, device=dev)
+    got = (_lib.c_i64 * 2)()
+    args = (vt, it, pt, nrows, ncols, nnz, ptr(indptr), ptr(indices), ptr(data))
+    _lib.check(L.b2s_csr_to_dia(*args, 0, 0, None, None, ptr(scratch), scratch.numel(), got, _stream()),
+               "b2s_csr_to_dia")
+    ndiag, Ld = int(got[0]), int(got[1])
+    allocate(ndiag, Ld)
+    offsets = torch.empty(ndiag, dtype=torch.int64, device=dev)
+    out = torch.empty((ndiag, Ld), dtype=data.dtype, device=dev)
+    if ndiag:
+            _lib.check(L.b2s_csr_to_dia(*args, ndiag, Ld, ptr(offsets), ptr(out), ptr(scratch), scratch.numel(), None,
+                                    _stream()), "b2s_csr_to_dia")
+    return offsets, out
+
+
 def spmv_tiles(indptr, indices, data, x, y, shape, plan, tile_lo: int, tile_hi: int):
     """Rows of tiles [tile_lo, tile_hi) of y = A @ x (x must be valid on that chunk's column window)."""
     _chk_dev(indptr, indices, data, x, y)

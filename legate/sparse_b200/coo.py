@@ -134,6 +134,10 @@ class coo_array:
 
         return csc_array(self)
 
+    def todia(self, copy=False):
+        """The DIA form of `tocsr()` (b2s_csr_to_dia on the GPU), as scipy's `todia`: repeated entries summed."""
+        return self.tocsr().todia()
+
     def todense(self):
         vals, i, j = self._host()
         out = np.zeros(self.shape, dtype=self.dtype)
@@ -175,4 +179,6 @@ class coo_array:
             return self.tocsr()
         if format == "csc":
             return self.tocsc()
+        if format == "dia":
+            return self.todia()
         raise NotImplementedError(f"format {format!r}")

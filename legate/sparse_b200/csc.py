@@ -20,6 +20,7 @@ import torch
 from . import _ops
 from .coo import coo_array
 from .csr import _dense_rows, csr_array
+from .dia import dia_array
 from .runtime import SUPPORTED_VALUE_DTYPES, numpy_dtype, runtime, to_device, to_host, torch_dtype
 
 
@@ -51,6 +52,8 @@ class csc_array:
             T = arg.transpose()
         elif isinstance(arg, coo_array):
             T = arg.transpose().tocsr()
+        elif isinstance(arg, dia_array):
+            T = arg.tocsr().transpose()
         elif isinstance(arg, tuple):
             if shape is None:
                 raise AssertionError("Cannot infer shape in this case.")
@@ -138,6 +141,10 @@ class csc_array:
     def tocoo(self, copy=False):
         return self._T.tocoo(copy=copy).transpose()
 
+    def todia(self, copy=False):
+        """The DIA form: that of `tocsr()` (b2s_csr_to_dia), new arrays whatever `copy` says."""
+        return self.tocsr().todia()
+
     def to_scipy_sparse_csc(self):
         return scipy.sparse.csc_array((to_host(self.data), to_host(self.indices), to_host(self.indptr)),
                                       shape=self.shape, dtype=self.dtype)
@@ -160,6 +167,8 @@ class csc_array:
             return self.tocsr(copy=copy)
         if format == "coo":
             return self.tocoo(copy=copy)
+        if format == "dia":
+            return self.todia(copy=copy)
         raise NotImplementedError(f"format {format!r}")
 
     def transpose(self, copy=False):

@@ -218,6 +218,12 @@ class csr_array:
 
         return csc_array(self)
 
+    def todia(self, copy=False):
+        """The DIA form (b2s_csr_to_dia on the GPU), as scipy's `todia`: new arrays whatever `copy` says."""
+        from .dia import _csr_to_dia
+
+        return _csr_to_dia(self)
+
     def tocoo(self, copy=False):
         from .coo import coo_array
 
@@ -498,8 +504,10 @@ class csr_array:
         if is_sparse_matrix(other) or scipy.sparse.issparse(other):
             from .csc import csc_array
 
-            if isinstance(other, csc_array):
-                # CSR x CSC is SpGEMM with the cached CSR form, not a dense product
+            from .dia import dia_array
+
+            if isinstance(other, (csc_array, dia_array)):
+                # CSR x CSC and CSR x DIA are SpGEMM with the cached CSR form, not a dense product
                 return self.dot(other.tocsr(), out=out)
             other = np.asarray(other.todense())
             other_originally_sparse = True

@@ -25,6 +25,14 @@ int check_csr(int it, int pt, int64_t nrows, int64_t ncols, int64_t nnz) {
   return B2S_OK;
 }
 
+int check_dia(int vt, int64_t nrows, int64_t ncols, int64_t ndiag, int64_t L) {
+  B2S_CHECK_ARG(vt == B2S_F32 || vt == B2S_F64, "bad value type code %d", vt);
+  B2S_CHECK_ARG(nrows >= 0 && ncols >= 0 && ndiag >= 0 && L >= 0, "negative dimension");
+  B2S_CHECK_ARG(L == 0 || ndiag <= INT64_MAX / 8 / L, "ndiag * L = %lld * %lld overflows int64", (long long)ndiag,
+                (long long)L);
+  return B2S_OK;
+}
+
 int get_props(DeviceProps* out) {
   static DeviceProps cache[64];
   static bool have[64] = {false};

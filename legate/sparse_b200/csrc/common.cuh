@@ -35,6 +35,9 @@ void set_error(const char* fmt, ...);
 // index and indptr type codes, no negative size, and an int32 indptr only below 2^31-1 entries.  Entry points without
 // an ncols or nnz argument pass 0.  Returns B2S_OK, or B2S_EINVAL with the message set.
 int check_csr(int it, int pt, int64_t nrows, int64_t ncols, int64_t nnz);
+// The DIA operand contract (include/b200sparse.h, DIA): a float32 / float64 value type code, no negative size, and
+// ndiag * L elements of at most 8 bytes addressable in int64.
+int check_dia(int vt, int64_t nrows, int64_t ncols, int64_t ndiag, int64_t L);
 
 // true when the byte ranges [p, p + bytes) and [q, q + qbytes) do not intersect (an empty or NULL range never does)
 inline bool disjoint(const void* p, int64_t bytes, const void* q, int64_t qbytes) {

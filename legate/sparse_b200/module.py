@@ -1,9 +1,9 @@
 """Construction: `diags`, `eye`, `identity`, `is_sparse_matrix`, and assembly from blocks: `kron`, `kronsum`, `bmat`,
 `hstack`, `vstack`, `block_diag`.
 
-`diags`, `eye` and `identity` follow the reference (sparse/module.py:96-246, sparse/dia.py:175-249: entries equal to
-zero are dropped by the `data != 0` mask, dia.py:236).  They are small assembly, not the hot path: built on the host
-(vectorised numpy, no scipy dependency in the arithmetic) and uploaded as a `csr_array`.
+`diags`, `spdiags`, `eye` and `identity` follow the reference (sparse/module.py:96-246, sparse/dia.py:175-249): the
+diagonals are laid out on the host as scipy lays them out and uploaded as a `dia_array`; their CSR and CSC forms are
+its device conversion, which drops entries equal to zero (the `data != 0` mask of dia.py:236).
 
 The block functions run on the device (csrc/construct.cu, DESIGN section 3.13): shapes, dtypes and the block table are
 worked out on the host from the operands' shapes alone, and two kernels write the result without reading anything back.
@@ -25,18 +25,21 @@ from . import _ops
 from .coo import coo_array
 from .csc import csc_array
 from .csr import _csr_binop, _index_dtype, _indptr_dtype, csr_array
-from .runtime import SUPPORTED_VALUE_DTYPES, runtime, to_host, torch_dtype
+from .dia import dia_array
+from .runtime import SUPPORTED_VALUE_DTYPES, runtime, to_device, to_host, torch_dtype
 
 
 def is_sparse_matrix(o) -> bool:
-    return isinstance(o, (csr_array, csc_array, coo_array))
+    return isinstance(o, (csr_array, csc_array, coo_array, dia_array))
 
 
-def _dia_to_csr(diagonals, offsets, shape, dtype):
+def _dia_data(diagonals, offsets, shape, dtype) -> np.ndarray:
+    """The ndiag x L data array of `diagonals` at `offsets`, laid out as scipy.sparse.diags_array lays it out: diagonal
+    k starts at column max(k, 0), and L is scipy's bound over the offsets."""
     m, n = shape
-    rows_l, cols_l, vals_l = [], [], []
-    for d, k in zip(diagonals, offsets):
-        k = int(k)
+    L = max([0] + [min(m + k, n - k) + max(0, k) for k in offsets])
+    data = np.zeros((len(offsets), L), dtype=dtype)
+    for j, (d, k) in enumerate(zip(diagonals, offsets)):
         length = min(m + min(k, 0), n - max(k, 0))
         if length <= 0:
             continue
@@ -46,45 +49,14 @@ def _dia_to_csr(diagonals, offsets, shape, dtype):
         if d.shape[0] < length:
             raise ValueError(f"Diagonal length (index {k}: {d.shape[0]} at offset {k}) does not agree with "
                              f"array size ({m}, {n}).")
-        d = d[:length]
-        i = np.arange(length, dtype=np.int64) + max(-k, 0)
-        j = i + k
-        keep = d != 0  # dia.tocsc drops explicit zeros (reference dia.py:236)
-        rows_l.append(i[keep]); cols_l.append(j[keep]); vals_l.append(d[keep])
-    if rows_l:
-        rows = np.concatenate(rows_l); cols = np.concatenate(cols_l); vals = np.concatenate(vals_l).astype(dtype)
-    else:
-        rows = cols = np.zeros(0, dtype=np.int64); vals = np.zeros(0, dtype=dtype)
-    return coo_array((vals, (rows, cols)), shape=shape).tocsr()
-
-
-class _dia_result:
-    """What `diags(...)` returns when no format is requested: supports `.tocsr()`, `.tocsc().T`,
-    `.todense()` -- the conversions the examples use (pde.py:163 `diags(...).tocsc().T`)."""
-
-    def __init__(self, csr):
-        self._csr = csr
-        self.shape = csr.shape
-        self.dtype = csr.dtype
-
-    def tocsr(self, copy=False):
-        return self._csr
-
-    def tocsc(self, copy=False):
-        return csc_array(self._csr)
-
-    def todense(self):
-        return self._csr.todense()
-
-    toarray = todense
-
-    @property
-    def T(self):
-        return _dia_result(self._csr.T)
+        data[j, max(k, 0):max(k, 0) + length] = d[:length]
+    return data
 
 
 def diags(diagonals, offsets=0, shape=None, format=None, dtype=None):
-    """scipy.sparse.diags signature (reference sparse/module.py:96-218)."""
+    """scipy.sparse.diags signature (reference sparse/module.py:96-218).  Returns a dia_array (format None or "dia")
+    whose data and offsets are those of scipy.sparse.diags_array, or its tocsr() / tocsc() ("csr", "csc"), which drop
+    entries equal to zero.  Repeated offsets are accepted and give repeated entries in the CSR form."""
     if np.isscalar(offsets):
         if len(diagonals) == 0 or np.isscalar(diagonals[0]):
             diagonals = [np.atleast_1d(diagonals)]
@@ -99,7 +71,7 @@ def diags(diagonals, offsets=0, shape=None, format=None, dtype=None):
         shape = (m, m)
     if dtype is None:
         dtype = np.result_type(*[np.asarray(d).dtype for d in diagonals])
-    m, n = shape
+    m, n = (int(s) for s in shape)
     full = []
     for d, k in zip(diagonals, offsets):
         length = min(m + min(k, 0), n - max(k, 0))
@@ -109,24 +81,38 @@ def diags(diagonals, offsets=0, shape=None, format=None, dtype=None):
         if d.shape[0] == 1 and length != 1:
             d = np.full(length, d[0])  # scalar broadcast, as scipy
         full.append(d)
-    csr = _dia_to_csr(full, offsets, (int(m), int(n)), np.dtype(dtype))
-    if format == "csr":
-        return csr
+    A = dia_array._from_parts(to_device(_dia_data(full, offsets, (m, n), np.dtype(dtype))), offsets, (m, n))
     if format in (None, "dia"):
-        return _dia_result(csr)
+        return A
+    if format == "csr":
+        return A.tocsr()
     if format == "csc":
-        return csc_array(csr)
+        return A.tocsc()
     raise NotImplementedError(f"diags(format={format!r})")
 
 
+def spdiags(data, diags, m=None, n=None, format=None):
+    """scipy.sparse.spdiags: the matrix with the rows of `data` on the diagonals `diags`, as
+    dia_array((data, diags), shape=(m, n)).asformat(format); (m, n) may be given as one tuple in m, and both default
+    to len(data[0])."""
+    if m is None and n is None:
+        m = n = len(data[0])
+    elif n is None:
+        m, n = m
+    return dia_array((data, diags), shape=(m, n)).asformat(format)
+
+
 def eye(m, n=None, k=0, dtype=np.float64, format=None):
-    """Reference sparse/module.py:221-246 (returns a CSR identity-like matrix)."""
+    """Reference sparse/module.py:221-246: a CSR identity-like matrix, or for format="dia" the dia_array scipy builds
+    (one diagonal of ones)."""
     if n is None:
         n = m
     m, n = int(m), int(n)
-    length = max(0, min(m + min(k, 0), n - max(k, 0)))
-    csr = _dia_to_csr([np.ones(length, dtype=dtype)], [k], (m, n), np.dtype(dtype))
-    return csr
+    if format == "dia":
+        return diags([np.ones(max(0, min(m + k, n)), dtype=dtype)], [k], shape=(m, n), dtype=dtype)
+    length = max(0, min(m + min(k, 0), n - max(k, 0)))   # a diagonal outside the matrix gives an empty one
+    data = _dia_data([np.ones(length, dtype=dtype)], [k], (m, n), np.dtype(dtype))
+    return dia_array._from_parts(to_device(data), [k], (m, n)).tocsr()
 
 
 def identity(n, dtype=np.float64, format=None):

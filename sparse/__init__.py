@@ -11,6 +11,8 @@ from legate.sparse_b200 import (  # noqa: F401
     csc_matrix,
     csr_array,
     csr_matrix,
+    dia_array,
+    dia_matrix,
     diags,
     eye,
     hstack,
@@ -21,6 +23,7 @@ from legate.sparse_b200 import (  # noqa: F401
     kronsum,
     linalg,
     runtime,
+    spdiags,
     vstack,
 )
 
