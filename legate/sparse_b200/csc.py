@@ -19,9 +19,10 @@ import torch
 
 from . import _ops
 from .coo import coo_array
-from .csr import _dense_rows, csr_array
+from ._dense import dense_dot
+from .csr import csr_array
 from .dia import dia_array
-from .runtime import SUPPORTED_VALUE_DTYPES, numpy_dtype, runtime, to_device, to_host, torch_dtype
+from .runtime import numpy_dtype, to_host
 
 
 def _swap_axis(axis):
@@ -198,57 +199,18 @@ class csc_array:
             if B.shape[0] != self.shape[1]:
                 raise ValueError(f"dimension mismatch: {self.shape} @ {B.shape}")
             return csc_array._wrap(B._T.dot(self._T))
-        x = other if isinstance(other, (np.ndarray, torch.Tensor)) else np.asarray(other)
-        if x.ndim not in (1, 2):
-            raise NotImplementedError("csc_array.dot: operand must be a vector, a dense 2-D array or a sparse matrix")
-        if x.shape[0] != self.shape[1]:
-            raise ValueError(f"dimension mismatch: {self.shape} @ {tuple(x.shape)}")
-        common = np.result_type(self.dtype, numpy_dtype(x.dtype))
-        if common.kind == "c":
-            if self.dtype.kind == "c":
-                return self.tocsr().dot(x, out=out)
-            return self._dot_complex(x, out, common)
-        vector = x.ndim == 1 or x.shape[1] == 1
-        if common not in SUPPORTED_VALUE_DTYPES:
-            raise NotImplementedError(f"{'SpMV' if vector else 'SpMM'} for resolved dtype {common} is not implemented "
-                                      "(float32/float64 kernels only)")
-        m, n = self.shape
-        rshape = (m,) if x.ndim == 1 else (m, x.shape[1])
-        _check_out(out, rshape, common)
-        runtime.require_cuda("csc_array.dot")
-        on_device = isinstance(x, torch.Tensor) and x.is_cuda
-        S = self._T._promoted(common)
-        if vector:
-            xd = to_device(x.reshape(-1), dtype=common)
-            direct = isinstance(out, torch.Tensor) and out.is_cuda and out.is_contiguous()
-            y = out.reshape(-1) if direct else torch.empty(m, dtype=torch_dtype(common), device=S.device)
-            _ops.spmv_csc(S._indptr, S._indices, S._data, xd, y, self.shape)
-            res = y.reshape(rshape)
-        else:
-            X = _dense_rows(x, common)
-            k = X.shape[1]
-            direct = (isinstance(out, torch.Tensor) and out.is_cuda and (k <= 1 or out.stride(1) == 1)
-                      and (m <= 1 or out.stride(0) >= k))
-            res = out if direct else torch.empty((m, k), dtype=torch_dtype(common), device=S.device)
-            _ops.spmm_csc(S._indptr, S._indices, S._data, X, res, self.shape)
-        return _deliver(res, out, on_device, direct)
 
-    def _dot_complex(self, x, out, common):
-        """A real A times a complex operand: the real SpMM of A on the (re, im)-interleaved view of x (twice the
-        columns), which is how complex arrays sit in memory."""
-        m, n = self.shape
-        rdt = np.dtype(np.float32) if common == np.complex64 else np.dtype(np.float64)
-        rshape = (m,) if x.ndim == 1 else (m, x.shape[1])
-        _check_out(out, rshape, common)
-        runtime.require_cuda("csc_array.dot")
-        on_device = isinstance(x, torch.Tensor) and x.is_cuda
-        X = to_device(x, dtype=common)
-        k = 1 if X.ndim == 1 else X.shape[1]
-        Xr = torch.view_as_real(X.reshape(n, k)).reshape(n, 2 * k)
-        S = self._T._promoted(rdt)
-        Yr = torch.empty((m, 2 * k), dtype=Xr.dtype, device=Xr.device)
-        _ops.spmm_csc(S._indptr, S._indices, S._data, Xr, Yr, self.shape)
-        return _deliver(torch.view_as_complex(Yr.reshape(m, k, 2)).reshape(rshape), out, on_device, False)
+        def spmv(dt, xd, y):
+            S = self._T._promoted(dt)
+            _ops.spmv_csc(S._indptr, S._indices, S._data, xd, y, self.shape)
+
+        def spmm(dt, X, Y):
+            S = self._T._promoted(dt)
+            _ops.spmm_csc(S._indptr, S._indices, S._data, X, Y, self.shape)
+
+        x = other if isinstance(other, (np.ndarray, torch.Tensor)) else np.asarray(other)
+        return dense_dot(x, out, self.dtype, self.shape, "csc_array.dot", spmv, spmm,
+                         lambda x, out: self.tocsr().dot(x, out=out))
 
     def matvec(self, other):
         return self @ other
@@ -384,26 +346,3 @@ def _as_csc_operand(other):
         if isinstance(csc, csc_array):
             return csc
     return None
-
-
-def _check_out(out, shape, dtype):
-    if out is None:
-        return
-    odt = numpy_dtype(out.dtype)
-    if odt != dtype:
-        raise ValueError(f"Output type {odt} is not consistent with resolved dtype {dtype}")
-    if tuple(out.shape) != tuple(shape):
-        raise ValueError(f"out has shape {tuple(out.shape)}, the result {tuple(shape)}")
-
-
-def _deliver(res, out, on_device, direct):
-    """The device result `res` in the caller's array kind: `out` when given (written unless the kernel wrote it
-    directly), else a CUDA tensor for a CUDA operand and numpy otherwise."""
-    if out is None:
-        return res if on_device else to_host(res)
-    if not direct:
-        if isinstance(out, torch.Tensor):
-            out.copy_(res)
-        else:
-            out[...] = to_host(res)
-    return out

@@ -23,9 +23,9 @@ import scipy.sparse
 import torch
 
 from . import _ops
+from ._dense import check_out, deliver, dense_dot, dense_rows, direct_out
 from .runtime import (
     SUPPORTED_VALUE_DTYPES,
-    is_device_array,
     numpy_dtype,
     runtime,
     to_device,
@@ -287,8 +287,9 @@ class csr_array:
 
     def _derived(self, kind, extra, build):
         """The derivative `kind` of the arrays (SpMV plan, promoted copy, transpose, ...) for the parameters `extra`:
-        `build()` runs again whenever the stamp or `extra` differs from the cached one.  One slot per kind, so a caller
-        switching parameters on one matrix does not pile up device buffers."""
+        `build()` runs again whenever `self._stamp()` or `extra` differs from the cached one.  One slot per kind, so a
+        caller switching parameters on one matrix does not pile up device buffers.  `dia_array` caches the same way,
+        against its own stamp."""
         stamp = self._stamp()
         hit = self._cache.get(kind)
         if hit is None or hit[0] != stamp or hit[1] != extra:
@@ -441,48 +442,29 @@ class csr_array:
         return csr_array._from_parts(e_ptr.to(_indptr_dtype(4 * nnz)), e_idx.to(_index_dtype(2 * n)), e_val,
                                      (2 * m, 2 * n))
 
-    def _dot_complex(self, other, out):
-        """A @ x / A @ X when the resolved dtype is complex (the reference dispatches its SpMV / SpMM tasks over
-        complex64/128 too, src/sparse/util/dispatch.h).  No complex kernels: a real A with a complex operand is the
-        real SpMM on the (re, im)-interleaved view of the operand (twice the columns); a complex A goes through its
-        real expansion (`_real_expansion`)."""
-        runtime.require_cuda("csr_array.dot")
-        assert self.shape[1] == other.shape[0]
+    def _dot_complex(self, x, out):
+        """A @ x for a complex A (the reference dispatches its SpMV / SpMM tasks over complex64/128 too,
+        src/sparse/util/dispatch.h).  No complex kernels: the real SpMV / SpMM of A's real expansion
+        (`_real_expansion`) on the (re, im)-interleaved view of x."""
         m, n = self.shape
-        common = np.result_type(self.dtype, numpy_dtype(other.dtype))
-        rdt = np.dtype(np.float32) if common == np.complex64 else np.dtype(np.float64)
-        if out is not None and numpy_dtype(out.dtype) != common:
-            raise ValueError(f"Output type {numpy_dtype(out.dtype)} is not consistent with resolved dtype {common}")
-        on_device = is_device_array(other) and other.is_cuda
-        X = to_device(other, dtype=common)
-        vector = X.ndim == 1
-        k = 1 if vector else X.shape[1]
+        common = np.result_type(self.dtype, numpy_dtype(x.dtype))
+        rshape = (m,) if x.ndim == 1 else (m, x.shape[1])
+        check_out(out, rshape, common)
+        runtime.require_cuda("csr_array.dot")
+        X = to_device(x, dtype=common)
+        k = 1 if X.ndim == 1 else X.shape[1]
         Xr = torch.view_as_real(X.reshape(n, k))                                  # (n, k, 2) real view
-        if self.dtype.kind != "c":
-            Ar = self._promoted(rdt)
-            Yr = torch.empty((m, 2 * k), dtype=Xr.dtype, device=Xr.device)
-            _ops.spmm(Ar._indptr, Ar._indices, Ar._data, Xr.reshape(n, 2 * k), Yr, Ar.shape)
-            Y = torch.view_as_complex(Yr.reshape(m, k, 2))
+        E = self._real_expansion(np.dtype(np.float32) if common == np.complex64 else np.dtype(np.float64))
+        if k == 1:
+            yr = torch.empty(2 * m, dtype=Xr.dtype, device=Xr.device)
+            _ops.spmv(E._indptr, E._indices, E._data, Xr.reshape(2 * n), yr, E.shape, plan=E._get_plan())
+            Y = torch.view_as_complex(yr.reshape(m, 1, 2))
         else:
-            E = self._real_expansion(rdt)
-            if k == 1:
-                yr = torch.empty(2 * m, dtype=Xr.dtype, device=Xr.device)
-                _ops.spmv(E._indptr, E._indices, E._data, Xr.reshape(2 * n), yr, E.shape, plan=E._get_plan())
-                Y = torch.view_as_complex(yr.reshape(m, 1, 2))
-            else:
-                Xe = Xr.permute(0, 2, 1).reshape(2 * n, k).contiguous()           # rows: re x_0, im x_0, re x_1, ...
-                Ye = torch.empty((2 * m, k), dtype=Xr.dtype, device=Xr.device)
-                _ops.spmm(E._indptr, E._indices, E._data, Xe, Ye, E.shape)
-                Y = torch.view_as_complex(Ye.reshape(m, 2, k).permute(0, 2, 1).contiguous())
-        Y = Y.reshape(m) if vector else Y.reshape(m, k)
-        if out is not None:
-            assert tuple(out.shape) == tuple(Y.shape)
-            if isinstance(out, torch.Tensor):
-                out.copy_(Y)
-            else:
-                out[...] = to_host(Y)
-            return out
-        return Y if on_device else to_host(Y)
+            Xe = Xr.permute(0, 2, 1).reshape(2 * n, k).contiguous()           # rows: re x_0, im x_0, re x_1, ...
+            Ye = torch.empty((2 * m, k), dtype=Xr.dtype, device=Xr.device)
+            _ops.spmm(E._indptr, E._indices, E._data, Xe, Ye, E.shape)
+            Y = torch.view_as_complex(Ye.reshape(m, 2, k).permute(0, 2, 1).contiguous())
+        return deliver(Y.reshape(rshape), out, isinstance(x, torch.Tensor) and x.is_cuda, False)
 
     def dot(self, other, out=None, spmv_domain_part=False):
         """`A.dot(x)` / `A @ B`; see reference sparse/csr.py:442-582.
@@ -501,7 +483,8 @@ class csr_array:
                 raise ValueError("Cannot provide out for CSRxCSR matmul.")
             assert self.shape[1] == other.shape[0]
             return spgemm_csr_csr_csr(*cast_to_common_type(self, other))
-        if is_sparse_matrix(other) or scipy.sparse.issparse(other):
+        densified = is_sparse_matrix(other) or scipy.sparse.issparse(other)
+        if densified:
             from .csc import csc_array
 
             from .dia import dia_array
@@ -510,115 +493,56 @@ class csr_array:
                 # CSR x CSC and CSR x DIA are SpGEMM with the cached CSR form, not a dense product
                 return self.dot(other.tocsr(), out=out)
             other = np.asarray(other.todense())
-            other_originally_sparse = True
-        else:
-            other_originally_sparse = False
-        if not isinstance(other, (np.ndarray, torch.Tensor)):
-            other = np.asarray(other)
-        if other.ndim in (1, 2) and np.result_type(self.dtype, numpy_dtype(other.dtype)).kind == "c":
-            res = self._dot_complex(other, out)
-            if other_originally_sparse:
-                return csr_array(np.asarray(to_host(res)).reshape(self.shape[0], -1))
-            return res
-        if other.ndim == 1 or (other.ndim == 2 and other.shape[1] == 1):
-            runtime.require_cuda("csr_array.dot")
-            assert self.shape[1] == other.shape[0]
-            on_device = is_device_array(other) and other.is_cuda
-            other_originally_2d = other.ndim == 2
-            x = other.reshape(-1) if other_originally_2d else other
-            if isinstance(x, torch.Tensor) and not x.is_contiguous():
+        x = other if isinstance(other, (np.ndarray, torch.Tensor)) else np.asarray(other)
+        res = self._dot_dense(x, out, spmv_domain_part)
+        if densified:
+            return csr_array(np.asarray(to_host(res)).reshape(self.shape[0], -1))
+        return res
+
+    def _dot_dense(self, x, out, spmv_domain_part):
+        """A @ x for a dense x: `dense_dot` with this class's launchers, after the checks the reference makes and the
+        software-pipelined product of host vectors (`_dot_host_pipelined`), which has to see x before it moves."""
+        m, n = self.shape
+        if x.ndim not in (1, 2):
+            raise NotImplementedError("csr_array.dot: operand must be a vector, a dense 2-D array or a csr_array")
+        rshape = (m,) if x.ndim == 1 else (m, x.shape[1])
+        assert x.shape[0] == n
+        assert out is None or tuple(out.shape) == rshape
+        common = np.result_type(self.dtype, numpy_dtype(x.dtype))
+        if (x.ndim == 1 or x.shape[1] == 1) and common.kind != "c":
+            if isinstance(x, torch.Tensor) and not x.reshape(-1).is_contiguous():
                 warnings.warn(
                     "CSR SpMV creating an implicit copy due to transformed x vector.",
                     category=RuntimeWarning,
-                    stacklevel=2,
+                    stacklevel=3,
                 )
-            xdt = numpy_dtype(x.dtype)
-            common = np.result_type(self.dtype, xdt)
-            if common not in SUPPORTED_VALUE_DTYPES:
-                raise NotImplementedError(
-                    f"SpMV for resolved dtype {common} is not implemented (float32/float64 kernels only)"
-                )
-            A = self._promoted(common)
-            if out is not None:
-                odt = numpy_dtype(out.dtype)
-                if odt != common:
-                    raise ValueError(f"Output type {odt} is not consistent with resolved dtype {common}")
-                if other_originally_2d:
-                    assert tuple(out.shape) == (self.shape[0], 1)
-                    assert not spmv_domain_part
-                else:
-                    assert tuple(out.shape) == (self.shape[0],)
-            plan = A._get_plan()
-            if (not on_device and isinstance(x, np.ndarray) and xdt == common and x.flags.c_contiguous
+            assert out is None or x.ndim == 1 or not spmv_domain_part
+            if (isinstance(x, np.ndarray) and x.dtype == common and common in SUPPORTED_VALUE_DTYPES
+                    and x.reshape(-1).flags.c_contiguous
                     and (out is None or (isinstance(out, np.ndarray) and out.flags.c_contiguous))
-                    and plan.chunks and not spmv_domain_part and os.environ.get("B2S_PIPELINE", "1") != "0"):
-                # host vectors: stream x in / y out chunk by chunk, overlapping both PCIe directions with the kernel
-                res = A._dot_host_pipelined(x, None if out is None else out.reshape(-1), plan)
-                result = out if out is not None else (res.reshape(-1, 1) if other_originally_2d else res)
-                if other_originally_sparse:
-                    return csr_array(np.asarray(result).reshape(self.shape[0], -1))
-                return result
-            xd = to_device(x, dtype=common)
-            direct = isinstance(out, torch.Tensor) and out.is_cuda and out.is_contiguous()
-            y = out.reshape(-1) if direct else torch.empty(self.shape[0], dtype=torch_dtype(common), device=A.device)
+                    and not spmv_domain_part and os.environ.get("B2S_PIPELINE", "1") != "0"):
+                check_out(out, rshape, common)
+                runtime.require_cuda("csr_array.dot")
+                A = self._promoted(common)
+                plan = A._get_plan()
+                if plan.chunks:
+                    # host vectors: stream x in / y out chunk by chunk, overlapping both PCIe directions with the kernel
+                    y = A._dot_host_pipelined(x.reshape(-1), None if out is None else out.reshape(-1), plan)
+                    return out if out is not None else y.reshape(rshape)
+
+        def spmv(dt, xd, y):
+            A = self._promoted(dt)
+            plan = A._get_plan()
             if spmv_domain_part or A._wants_col_split(plan):
                 A._dot_col_split(xd, y)      # x partitioned by columns, partial products reduced into y
             else:
                 _ops.spmv(A._indptr, A._indices, A._data, xd, y, A.shape, plan=plan)
-            if out is None:
-                result = y if on_device else to_host(y)
-                if other_originally_2d:
-                    result = result.reshape(-1, 1)
-            else:
-                if not direct:
-                    if isinstance(out, torch.Tensor):
-                        out.reshape(-1).copy_(y)
-                    else:
-                        flat = out.reshape(-1)
-                        if flat.flags.c_contiguous and np.shares_memory(flat, out):
-                            torch.from_numpy(flat).copy_(y)  # D2H straight into the caller's (pinned) buffer
-                        else:
-                            flat[...] = to_host(y)
-                result = out
-            if other_originally_sparse:
-                return csr_array(np.asarray(to_host(result)).reshape(self.shape[0], -1))
-            return result
-        if other.ndim == 2:
-            # SpMM, reference csr.py:552-579: C = A @ B with a dense row-major B; `out` must have the resolved dtype.
-            runtime.require_cuda("csr_array.dot")
-            assert self.shape[1] == other.shape[0]
-            on_device = is_device_array(other) and other.is_cuda
-            common = np.result_type(self.dtype, numpy_dtype(other.dtype))
-            if common not in SUPPORTED_VALUE_DTYPES:
-                raise NotImplementedError(
-                    f"SpMM for resolved dtype {common} is not implemented (float32/float64 kernels only)"
-                )
-            A = self._promoted(common)
-            k = other.shape[1]
-            if out is not None:
-                odt = numpy_dtype(out.dtype)
-                if odt != common:
-                    raise ValueError(f"Output type {odt} is not consistent with resolved dtype {common}")
-                assert tuple(out.shape) == (self.shape[0], k)
-            B = to_device(other, dtype=common)
-            if k > 1 and B.stride(1) != 1:
-                B = B.contiguous()  # transposed / column-strided operand: the kernel needs contiguous rows (csr.py:572-577)
-            direct = isinstance(out, torch.Tensor) and out.is_cuda and (k <= 1 or out.stride(1) == 1)
-            C = out if direct else torch.empty((self.shape[0], k), dtype=torch_dtype(common), device=A.device)
-            _ops.spmm(A._indptr, A._indices, A._data, B, C, A.shape)
-            if out is None:
-                result = C if on_device else to_host(C)
-            else:
-                if not direct:
-                    if isinstance(out, torch.Tensor):
-                        out.copy_(C)
-                    else:
-                        out[...] = to_host(C)
-                result = out
-            if other_originally_sparse:
-                return csr_array(np.asarray(to_host(result)))
-            return result
-        raise NotImplementedError("csr_array.dot: operand must be a vector, a dense 2-D array or a csr_array")
+
+        def spmm(dt, X, Y):
+            A = self._promoted(dt)
+            _ops.spmm(A._indptr, A._indices, A._data, X, Y, A.shape)
+
+        return dense_dot(x, out, self.dtype, self.shape, "csr_array.dot", spmv, spmm, self._dot_complex)
 
     def matvec(self, other):
         return self @ other
@@ -760,8 +684,8 @@ class csr_array:
             raise NotImplementedError(f"sddmm for dtype {common} is not implemented (float32/float64 kernels only)")
         runtime.require_cuda("csr_array.sddmm")
         A = self._promoted(common)
-        Cd = _dense_rows(Cx, common)
-        Dt = _dense_rows(Dx.T, common)
+        Cd = dense_rows(Cx, common)
+        Dt = dense_rows(Dx.T, common)
         out = _ops.sddmm(A._indptr, A._indices, A._data, Cd, Dt)
         return csr_array._from_parts(A._indptr, A._indices, out, self.shape)
 
@@ -795,19 +719,9 @@ class csr_array:
             if _overlaps(out, x):
                 raise ValueError("out overlaps the operand of tropical_spmv")
         runtime.require_cuda("csr_array.tropical_spmv")
-        on_device = is_device_array(x) and x.is_cuda
-        xd = _dense_rows(x, np.int64)
-        direct = (isinstance(out, torch.Tensor) and out.is_cuda and (nf <= 1 or m == 0 or out.stride(1) == 1)
-                  and (m <= 1 or out.stride(0) >= nf))
-        y = _ops.tropical_spmv(self._indptr, self._indices, xd, out if direct else None)
-        if out is None:
-            return y if on_device else to_host(y)
-        if not direct:
-            if isinstance(out, torch.Tensor):
-                out.copy_(y)
-            else:
-                out[...] = to_host(y)
-        return out
+        direct = direct_out(out, (m, nf))
+        y = _ops.tropical_spmv(self._indptr, self._indices, dense_rows(x, np.int64), out if direct else None)
+        return deliver(y, out, isinstance(x, torch.Tensor) and x.is_cuda, direct)
 
     # -- reductions (scipy csr_array sum / mean / max / min / argmax / argmin / count_nonzero; csrc/reduce.cu) ----------
     def _canonical(self):
@@ -862,7 +776,7 @@ class csr_array:
         if axis is None:
             return _deliver_scalar(rdt.type(float(A._data.sum(dtype=torch.float64))), out)
         v = A._reduce_axis("sum", axis)
-        return _deliver_vector(v.to(torch_dtype(rdt)), out)
+        return deliver(v.to(torch_dtype(rdt)), out, True, False)
 
     def mean(self, axis=None, dtype=None, out=None):
         """`sum(axis, dtype)` divided by shape[axis] (by m * n for axis None); same result kinds and `out` as sum."""
@@ -874,7 +788,7 @@ class csr_array:
         if axis is None:
             with np.errstate(invalid="ignore", divide="ignore"):
                 return _deliver_scalar(rdt.type(np.true_divide(s, rdt.type(count))), out)
-        return _deliver_vector(s / count, out)
+        return deliver(s / count, out, True, False)
 
     def _reduction_dtype(self, dtype, what):
         rdt = self.dtype if dtype is None else np.dtype(dtype)
@@ -1283,28 +1197,6 @@ def _deliver_scalar(value, out):
     else:
         out[...] = value
     return out
-
-
-def _deliver_vector(v, out):
-    if out is None:
-        return v
-    if isinstance(out, torch.Tensor):
-        out.copy_(v)
-    else:
-        out[...] = to_host(v)
-    return out
-
-
-def _dense_rows(a, dtype):
-    """A 2-D operand as a device tensor of `dtype` whose rows are unit-stride and do not overlap (the row stride may be
-    larger than a row): a tensor already in that form is used without a copy."""
-    if not isinstance(a, torch.Tensor):
-        return to_device(a, dtype=dtype)   # numpy: C-ordered (a view when it already is) and copied to the device
-    t = a.to(device=runtime.device, dtype=torch_dtype(dtype))
-    rows, k = t.shape
-    if (k > 1 and t.stride(1) != 1) or (rows > 1 and t.stride(0) < k):
-        t = t.contiguous()
-    return t
 
 
 def _is_integer_dtype(dt) -> bool:

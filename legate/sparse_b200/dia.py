@@ -20,8 +20,9 @@ import scipy.sparse
 import torch
 
 from . import _ops
-from .csr import _dense_rows, _index_dtype, _indptr_dtype, csr_array
-from .runtime import SUPPORTED_VALUE_DTYPES, numpy_dtype, runtime, to_device, to_host, torch_dtype
+from ._dense import dense_dot
+from .csr import _as_sparse_operand, _index_dtype, _indptr_dtype, csr_array
+from .runtime import numpy_dtype, runtime, to_device, to_host, torch_dtype
 
 _DIA_WARN_DIAGONALS = 100   # scipy's coo.todia warns above this many diagonals
 
@@ -146,13 +147,7 @@ class dia_array:
         The offsets never change after construction."""
         return self._data.data_ptr(), self._data._version
 
-    def _derived(self, kind, extra, build):
-        """As `csr_array._derived`: `build()` runs again whenever the stamp or `extra` differs from the cached one."""
-        stamp = self._stamp()
-        hit = self._cache.get(kind)
-        if hit is None or hit[0] != stamp or hit[1] != extra:
-            hit = self._cache[kind] = (stamp, extra, build())
-        return hit[2]
+    _derived = csr_array._derived
 
     def _in_band(self):
         """(offsets, data) restricted to the diagonals that meet the band -- -m < k < min(n, L) -- with the offsets as
@@ -313,68 +308,23 @@ class dia_array:
         np.result_type of A and x; float32 and float64 run the kernels, a complex operand runs the real SpMM on the
         (re, im)-interleaved view (a complex A runs the complex CSR path of `tocsr()`), and anything else raises
         NotImplementedError."""
-        from .csc import _check_out, _deliver
-
-        B = _as_csr_operand(other)
+        B = _as_sparse_operand(other)
         if B is not None:
             if out is not None:
                 raise ValueError("Cannot provide out for sparse matmul.")
             if B.shape[0] != self.shape[1]:
                 raise ValueError(f"dimension mismatch: {self.shape} @ {B.shape}")
             return self.tocsr().dot(B)
+
+        def spmv(dt, xd, y):
+            _ops.spmv_dia(*self._promoted(dt)._in_band(), xd, y, self.shape)
+
+        def spmm(dt, X, Y):
+            _ops.spmm_dia(*self._promoted(dt)._in_band(), X, Y, self.shape)
+
         x = other if isinstance(other, (np.ndarray, torch.Tensor)) else np.asarray(other)
-        if x.ndim not in (1, 2):
-            raise NotImplementedError("dia_array.dot: operand must be a vector, a dense 2-D array or a sparse matrix")
-        if x.shape[0] != self.shape[1]:
-            raise ValueError(f"dimension mismatch: {self.shape} @ {tuple(x.shape)}")
-        common = np.result_type(self.dtype, numpy_dtype(x.dtype))
-        if common.kind == "c":
-            if self.dtype.kind == "c":
-                return self.tocsr().dot(x, out=out)
-            return self._dot_complex(x, out, common)
-        vector = x.ndim == 1 or x.shape[1] == 1
-        if common not in SUPPORTED_VALUE_DTYPES:
-            raise NotImplementedError(f"{'SpMV' if vector else 'SpMM'} for resolved dtype {common} is not implemented "
-                                      "(float32/float64 kernels only)")
-        m, n = self.shape
-        rshape = (m,) if x.ndim == 1 else (m, x.shape[1])
-        _check_out(out, rshape, common)
-        runtime.require_cuda("dia_array.dot")
-        on_device = isinstance(x, torch.Tensor) and x.is_cuda
-        offsets, data = self._promoted(common)._in_band()
-        if vector:
-            xd = to_device(x.reshape(-1), dtype=common)
-            direct = isinstance(out, torch.Tensor) and out.is_cuda and out.is_contiguous()
-            y = out.reshape(-1) if direct else torch.empty(m, dtype=torch_dtype(common), device=data.device)
-            _ops.spmv_dia(offsets, data, xd, y, self.shape)
-            res = y.reshape(rshape)
-        else:
-            X = _dense_rows(x, common)
-            k = X.shape[1]
-            direct = (isinstance(out, torch.Tensor) and out.is_cuda and (k <= 1 or out.stride(1) == 1)
-                      and (m <= 1 or out.stride(0) >= k))
-            res = out if direct else torch.empty((m, k), dtype=torch_dtype(common), device=data.device)
-            _ops.spmm_dia(offsets, data, X, res, self.shape)
-        return _deliver(res, out, on_device, direct)
-
-    def _dot_complex(self, x, out, common):
-        """A real A times a complex operand: the real SpMM of A on the (re, im)-interleaved view of x (twice the
-        columns), which is how complex arrays sit in memory."""
-        from .csc import _check_out, _deliver
-
-        m, n = self.shape
-        rdt = np.dtype(np.float32) if common == np.complex64 else np.dtype(np.float64)
-        rshape = (m,) if x.ndim == 1 else (m, x.shape[1])
-        _check_out(out, rshape, common)
-        runtime.require_cuda("dia_array.dot")
-        on_device = isinstance(x, torch.Tensor) and x.is_cuda
-        X = to_device(x, dtype=common)
-        k = 1 if X.ndim == 1 else X.shape[1]
-        Xr = torch.view_as_real(X.reshape(n, k)).reshape(n, 2 * k)
-        offsets, data = self._promoted(rdt)._in_band()
-        Yr = torch.empty((m, 2 * k), dtype=Xr.dtype, device=Xr.device)
-        _ops.spmm_dia(offsets, data, Xr, Yr, self.shape)
-        return _deliver(torch.view_as_complex(Yr.reshape(m, k, 2)).reshape(rshape), out, on_device, False)
+        return dense_dot(x, out, self.dtype, self.shape, "dia_array.dot", spmv, spmm,
+                         lambda x, out: self.tocsr().dot(x, out=out))
 
     def matvec(self, other):
         return self @ other
@@ -456,17 +406,6 @@ class dia_array:
 
 
 dia_matrix = dia_array
-
-
-def _as_csr_operand(other):
-    """`other` as a csr_array when it is a sparse matrix of this library or of scipy, else None."""
-    from .module import is_sparse_matrix
-
-    if isinstance(other, csr_array):
-        return other
-    if is_sparse_matrix(other) or scipy.sparse.issparse(other):
-        return csr_array(other)
-    return None
 
 
 def _csr_to_dia(A: csr_array) -> dia_array:
