@@ -268,7 +268,8 @@ int         b2s_csr_diagonal(int vt, int it, int pt, int64_t nrows, const void* 
  * Pass 2 (numeric): fills c_indices (int32) / c_vals; rows come out SORTED by column
  *   (canonical form; reference/scipy rows are unsorted, compare after sort_indices()).
  *   Structural zeros from cancellation are kept, as in the reference.
- * `scratch`: device buffer of b2s_spgemm_scratch_bytes(m, n) bytes shared by both passes.
+ * `scratch`: device buffer of b2s_spgemm_scratch_bytes(m, n) bytes shared by both passes: O(m) bytes plus the
+ *   dense rows' bitmap slots of about n/8 bytes each, 4 per SM but no more than 1 GiB of them (at least one).
  * `dense_ws`: device buffer of b2s_spgemm_dense_bytes(vt, n, info_host[2]) bytes (may be
  *   NULL when that is 0) -- the parallel form of the reference's per-thread `workspace` /
  *   `already_set` arrays (spgemm_csr_csr_csr.cc:100-118, _omp.cc:92-167). */

@@ -1027,7 +1027,8 @@ def spgemm_csr_csr_csr(A: csr_array, B: csr_array) -> csr_array:
     if a_ptr.dtype != b_ptr.dtype:
         a_ptr, b_ptr = a_ptr.to(torch.int64), b_ptr.to(torch.int64)
     c_ptr, c_idx, c_val, info = _ops.spgemm(a_ptr, a_idx, A._data, b_ptr, b_idx, B._data, A.shape, B.shape)
-    C = csr_array._from_parts(c_ptr.to(_indptr_dtype(info["nnz"])), c_idx, c_val, (A.shape[0], B.shape[1]))
+    C = csr_array._from_parts(c_ptr.to(_indptr_dtype(info["nnz"])), c_idx.to(_index_dtype(B.shape[1] - 1)), c_val,
+                              (A.shape[0], B.shape[1]))
     C.spgemm_info = info
     return C
 

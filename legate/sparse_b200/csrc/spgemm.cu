@@ -12,8 +12,9 @@
 //              `workspace`/`already_set` pair) -> rows are emitted SORTED by column.
 //
 // Like the reference (and scipy) the structure is symbolic: cancellation zeros are kept.  Integer /
-// HBM-latency bound work: no tensor cores.  Within the warp-per-row bins the A-row is walked in order and
-// lanes cover one B-row at a time, so per-column accumulation order equals the reference's Gustavson order.
+// HBM-latency bound work: no tensor cores.  Within the warp-per-row bins the products are enumerated in the reference's
+// Gustavson (A entry, B entry) order, 32 per round; the products of one column within a round are summed first and that
+// sum is added to the column's slot, so the result is deterministic but not the reference's left-to-right sum.
 #include "common.cuh"
 #include <limits.h>
 
@@ -63,7 +64,15 @@ static ScratchLayout scratch_layout(int64_t m, int64_t n, int sm_count) {
   L.bitmap_words0 = (n + 31) / 32;
   L.bitmap_words1 = (L.bitmap_words0 + 31) / 32;
   L.bitmap_slot_bytes = align_up(4 * (L.bitmap_words0 + L.bitmap_words1), 256);
-  L.nslots = 4 * sm_count;   // dense-row CTAs resident at once (28 registers: the accumulators are the limit, not the SM)
+  // one slot per dense-row CTA resident at once (28 registers: the accumulators are the limit, not the SM), within a byte
+  // budget: a slot is n/8 bytes, and 4 x 132 SMs of them would take 136 GiB at n = 2^31 - 2, dense rows or not.  The
+  // dense kernel takes rows from a ticket counter, so any slot count >= 1 is correct.  The budget keeps every slot up to
+  // n ~ 16 M columns on 132 SMs, and beyond that still allows at least as many slots as the 24 GiB accumulator budget of
+  // b2s_spgemm_dense_bytes does, so only the symbolic pass of matrices that wide runs fewer dense-row CTAs.
+  constexpr int64_t BITMAP_BUDGET = 1LL << 30;
+  L.nslots = 4 * sm_count;
+  if (L.bitmap_slot_bytes * L.nslots > BITMAP_BUDGET)
+    L.nslots = (int)(BITMAP_BUDGET / L.bitmap_slot_bytes > 1 ? BITMAP_BUDGET / L.bitmap_slot_bytes : 1);
   L.off_bitmaps = o;   o += L.bitmap_slot_bytes * L.nslots;
   L.total = o;
   return L;
@@ -371,8 +380,9 @@ spgemm_warp_kernel(int64_t count, const int32_t* __restrict__ perm, const P* __r
           if (NUMERIC) prod = o_av * b_val[jb];
         }
         if (NUMERIC) {
-          // lanes that hit the same column are summed by the lowest of them in lane (= product) order, so the
-          // result is deterministic and follows the reference's accumulation order; no atomics on the values
+          // lanes that hit the same column are summed by the lowest of them in lane (= product) order and the sum is
+          // added to the slot: deterministic, but a round's partial sum is formed before it meets the slot's running
+          // value, which the reference's left-to-right order does not do; no atomics on the values
           const unsigned m = __match_any_sync(0xffffffffu, slot);
           const int leader = __ffs(m) - 1;
           unsigned rem = m;
