@@ -912,19 +912,58 @@ spmv_rowgroup_kernel(int64_t nrows, const P* __restrict__ indptr, const I* __res
 // ---------------------------------------------------------------------------------------------
 // Row templates (TemplateTable): y[r] = sum_j val[t][j] * x[r + off[t][j]] with t = ids[r].  No matrix stream but one
 // byte per row, so no staging ring either: the table sits in shared memory, a warp takes chunks of 32 R consecutive
-// rows (lane l: rows l + 32 q) and issues the gathers of all its R rows before the first FMA.  A grid of resident CTAs
-// walks the chunks in row order, so the rows in flight span a few MB of x and its +-n1 neighbours stay in L2.
+// rows (lane l: rows l + 32 q).  A grid of resident CTAs walks the chunks in row order, so the rows in flight span a
+// few MB of x and its +-n1 neighbours stay in L2.
+// Software pipeline of depth D over each warp's chunks c_i = c_0 + i S (S = gridDim.x * warps per CTA): while chunk i
+// is summed and stored, the x gathers of chunks i+1 .. i+D-1 and the ids of chunks up to i+D+1 are already in flight.
+// Without it a chunk costs two dependent memory trips (its ids, then its gathers) with nothing else outstanding in the
+// warp.  The ids of a chunk are loaded two steps before its gathers, its gathers D-1 steps before its sum.  Chunks
+// past the end load nothing (their rows are all >= nrows).  Both rings are indexed by compile-time slots of a loop
+// unrolled NT times, so no value moves between registers while its load is still pending.
 // Each sum is formed exactly as the one-lane-per-row CSR path forms it (short_row_sum: U terms from +0 in stored order,
 // zero products past the row's end, then + 0.0 in place of the old y), so y is bit-identical to the other kernels of
 // the same plan -- up to which NaN survives where two different NaNs meet in one FMA (an inf - inf sum times a NaN in
 // x), which follows the operand order the compiler picked for that FMA.
 // ---------------------------------------------------------------------------------------------
-// 64 warps per SM: at most 32 registers.
-template <typename V, int U, int R, int THREADS, bool DOT>
-__global__ void __launch_bounds__(THREADS, 2048 / THREADS)
+template <int R>
+__device__ __forceinline__ void tpl_load_ids(int (&t)[R], const uint8_t* __restrict__ ids, int64_t c, int64_t nrows,
+                                             int lane) {
+#pragma unroll
+  for (int q = 0; q < R; q++) {
+    const int64_t r = c * (32 * R) + 32 * q + lane;
+    t[q] = r < nrows ? (int)__ldcs(ids + r) : 0;
+  }
+}
+
+template <typename V, int U, int R>
+__device__ __forceinline__ void tpl_gather(V (&xv)[R][U], const int (&t)[R], const int (*soff)[U], const int* slen,
+                                           const V* __restrict__ x, int64_t c, int64_t nrows, int lane) {
+#pragma unroll
+  for (int q = 0; q < R; q++) {
+    const int64_t r = c * (32 * R) + 32 * q + lane;
+    const int n = r < nrows ? slen[t[q]] : 0;
+#pragma unroll
+    for (int j = 0; j < U; j++) xv[q][j] = j < n ? __ldg(x + (r + soff[t[q]][j])) : (V)0;
+  }
+}
+
+// Pipeline depth D (chunks whose gathers are in flight, the one being summed included) and CTAs of 256 threads per SM
+// the launch bound asks for: the sweep in DESIGN.md 8 (tools/sweep_templates.py).  On an H100 at 700 W, loading the ids
+// ahead (D = 1) was fastest for fp64 and fp32, with and without the fused dot; deeper rings gained nothing once fp64 L5
+// ran at the copy ceiling, and cost occupancy (the fp64 dot: 168-170 us against 153 on pde.py's operator).  No bound
+// spills: fp64 products of rows of up to 5 entries keep the 32 registers of 8 CTAs (the fastest), the fused dot 46-48 (5
+// CTAs; 8 CTAs lose 1.5 %), the rest 40 (6 CTAs), and two rows per lane 48 or, with the fp64 dot, 64 (4 CTAs).
+template <typename V, int U, int R, bool DOT> struct TplPipe {
+  static constexpr int D = 1;
+  static constexpr int MINB = R == 2 ? (DOT && sizeof(V) == 8 ? 4 : 5) : DOT ? 5 : (U == 5 && sizeof(V) == 8 ? 8 : 6);
+};
+
+template <typename V, int U, int R, int THREADS, int D, int MINB, bool DOT>
+__global__ void __launch_bounds__(THREADS, MINB)
 spmv_template_kernel(int64_t nrows, const uint8_t* __restrict__ ids, const TemplateTable* __restrict__ tab,
                      const V* __restrict__ x, V* __restrict__ y, int streaming, const V* __restrict__ w, V* dot_out,
                      void* ws) {
+  static_assert(D >= 1 && D <= 3, "pipeline depth 1..3");
   __shared__ int soff[kMaxTemplates][U];
   __shared__ V sval[kMaxTemplates][U];
   __shared__ int slen[kMaxTemplates];
@@ -940,36 +979,42 @@ spmv_template_kernel(int64_t nrows, const uint8_t* __restrict__ ids, const Templ
   if (threadIdx.x < kMaxTemplates) slen[threadIdx.x] = tab->len[threadIdx.x];
   __syncthreads();
   constexpr int WPB = THREADS / 32;
+  // id ring: chunks i .. i+D+1 are live at step i; a multiple of D so that one unrolled pass returns both rings to slot 0
+  constexpr int NT = D * ((D + 2 + D - 1) / D);
   const int lane = threadIdx.x & 31;
   const int64_t nchunks = (nrows + 32 * R - 1) / (32 * R);
+  const int64_t S = (int64_t)gridDim.x * WPB;
+  int64_t c = (int64_t)blockIdx.x * WPB + (threadIdx.x >> 5);
+  int t[NT][R];
+  V xv[D][R][U];
+#pragma unroll
+  for (int k = 0; k <= D; k++) tpl_load_ids<R>(t[k], ids, c + k * S, nrows, lane);
+#pragma unroll
+  for (int k = 0; k < D - 1; k++) tpl_gather<V, U, R>(xv[k], t[k], soff, slen, x, c + k * S, nrows, lane);
   double dot_acc = 0.0;
-  for (int64_t c = (int64_t)blockIdx.x * WPB + (threadIdx.x >> 5); c < nchunks; c += (int64_t)gridDim.x * WPB) {
-    const int64_t r0 = c * (32 * R) + lane;
-    int t[R], n[R];
+  while (c < nchunks) {
 #pragma unroll
-    for (int q = 0; q < R; q++) {
-      const int64_t r = r0 + 32 * q;
-      t[q] = r < nrows ? (int)__ldcs(ids + r) : 0;
-      n[q] = r < nrows ? slen[t[q]] : 0;
-    }
-    V xv[R][U];
+    for (int k = 0; k < NT; k++) {
+      if (c >= nchunks) break;
+      tpl_gather<V, U, R>(xv[(k + D - 1) % D], t[(k + D - 1) % NT], soff, slen, x, c + (D - 1) * S, nrows, lane);
+      tpl_load_ids<R>(t[(k + D + 1) % NT], ids, c + (D + 1) * S, nrows, lane);
+      const int (&tc)[R] = t[k % NT];
+      const V (&xc)[R][U] = xv[k % D];
 #pragma unroll
-    for (int q = 0; q < R; q++) {
+      for (int q = 0; q < R; q++) {
+        const int64_t r = c * (32 * R) + 32 * q + lane;
+        const int n = r < nrows ? slen[tc[q]] : 0;
+        V acc = (V)0;
 #pragma unroll
-      for (int j = 0; j < U; j++) xv[q][j] = j < n[q] ? __ldg(x + (r0 + 32 * q + soff[t[q]][j])) : (V)0;
-    }
-#pragma unroll
-    for (int q = 0; q < R; q++) {
-      V acc = (V)0;
-#pragma unroll
-      for (int j = 0; j < U; j++) acc += (j < n[q] ? sval[t[q]][j] : (V)0) * xv[q][j];
-      acc += (V)0;   // the CSR path's "+ old y" of a plain product: -0.0 -> +0.0 exactly as there
-      const int64_t r = r0 + 32 * q;
-      if (r < nrows) {
-        if (streaming) __stcs(y + r, acc);
-        else           y[r] = acc;
-        if (DOT) dot_acc += (double)acc * (double)w[r];
+        for (int j = 0; j < U; j++) acc += (j < n ? sval[tc[q]][j] : (V)0) * xc[q][j];
+        acc += (V)0;   // the CSR path's "+ old y" of a plain product: -0.0 -> +0.0 exactly as there
+        if (r < nrows) {
+          if (streaming) __stcs(y + r, acc);
+          else           y[r] = acc;
+          if (DOT) dot_acc += (double)acc * (double)w[r];
+        }
       }
+      c += S;
     }
   }
   if (DOT) {
@@ -1156,9 +1201,9 @@ static int dispatch_rowgroup(int it, int pt, int64_t nrows, int64_t nnz, const v
 }
 
 // Row-template launches: one resident wave of CTAs (occupancy x SMs) walking the row chunks in order.
-template <typename V, int U, int R, int THREADS, bool DOT>
+template <typename V, int U, int R, int THREADS, int D, int MINB, bool DOT>
 static int launch_template_f(const TemplateLaunch& a) {
-  auto kern = spmv_template_kernel<V, U, R, THREADS, DOT>;
+  auto kern = spmv_template_kernel<V, U, R, THREADS, D, MINB, DOT>;
   static LaunchCache cache;
   int occ = 1;
   if (int rc = launch_prepare(cache, kern, THREADS, 0, &occ)) return rc;
@@ -1176,18 +1221,24 @@ static int launch_template_f(const TemplateLaunch& a) {
   return B2S_OK;
 }
 
+template <typename V, int U, int R, int THREADS, bool DOT>
+static int launch_template_p(const TemplateLaunch& a) {
+  using P = TplPipe<V, U, R, DOT>;
+  return launch_template_f<V, U, R, THREADS, P::D, P::MINB * 256 / THREADS, DOT>(a);
+}
+
 // Instantiated: rows of up to 5 entries at R in {1, 2} and 128 / 256 threads (the sweep in DESIGN.md 8); longer rows
-// (up to kTplLen) at one row per lane and 256 threads whatever the tuning hook asks, so they keep 64 warps per SM.
+// (up to kTplLen) at one row per lane and 256 threads whatever the tuning hook asks.
 template <typename V, bool DOT>
 static int launch_template(const TemplateLaunch& a) {
   if (a.maxlen > 5) {
-    return launch_template_f<V, kTplLen, 1, 256, DOT>(a);
+    return launch_template_p<V, kTplLen, 1, 256, DOT>(a);
   } else if (a.threads == 256) {
-    if (a.rows == 1) return launch_template_f<V, 5, 1, 256, DOT>(a);
-    if (a.rows == 2) return launch_template_f<V, 5, 2, 256, DOT>(a);
+    if (a.rows == 1) return launch_template_p<V, 5, 1, 256, DOT>(a);
+    if (a.rows == 2) return launch_template_p<V, 5, 2, 256, DOT>(a);
   } else if (a.threads == 128) {
-    if (a.rows == 1) return launch_template_f<V, 5, 1, 128, DOT>(a);
-    if (a.rows == 2) return launch_template_f<V, 5, 2, 128, DOT>(a);
+    if (a.rows == 1) return launch_template_p<V, 5, 1, 128, DOT>(a);
+    if (a.rows == 2) return launch_template_p<V, 5, 2, 128, DOT>(a);
   }
   set_error("no row-template kernel is built for %d rows per lane, %d threads and rows of %d entries", a.rows, a.threads,
             a.maxlen);

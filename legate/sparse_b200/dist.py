@@ -636,7 +636,7 @@ class dist_csr_array:
         A = self.local
         if out is None:
             out = torch.empty(A.shape[0], dtype=x_full.dtype, device=x_full.device)
-        xin = x_full[: A.shape[1]]
+        xin = x_full if x_full.shape[0] == A.shape[1] else x_full[: A.shape[1]]
         if self.use_fused and x_full.is_cuda and self.exchange_mode != "none":
             info = self._fused_setup(A, x_full)
             if info is not None:

@@ -46,6 +46,9 @@ def numpy_dtype(dt) -> np.dtype:
 
 
 def vt_code(dt) -> int:
+    code = _VT_OF_TORCH.get(dt) if isinstance(dt, torch.dtype) else None
+    if code is not None:   # every launch asks: skip the numpy dtype comparisons
+        return code
     dt = numpy_dtype(dt)
     if dt == np.float32:
         return _lib.F32
@@ -58,12 +61,19 @@ def vt_code(dt) -> int:
 
 
 def idx_code(dt) -> int:
+    code = _IDX_OF_TORCH.get(dt) if isinstance(dt, torch.dtype) else None
+    if code is not None:
+        return code
     dt = numpy_dtype(dt)
     if dt == np.int32:
         return _lib.I32
     if dt == np.int64:
         return _lib.I64
     raise TypeError(f"index arrays must be int32 or int64, got {dt}")
+
+
+_VT_OF_TORCH = {torch.float32: _lib.F32, torch.float64: _lib.F64}
+_IDX_OF_TORCH = {torch.int32: _lib.I32, torch.int64: _lib.I64}
 
 
 class Runtime:
@@ -97,7 +107,9 @@ class Runtime:
             )
 
     def stream_ptr(self) -> int:
-        return torch.cuda.current_stream().cuda_stream
+        # the raw handle, without building a torch.cuda.Stream object: every launch asks, and at SpMV sizes the
+        # object costs as much host time as the rest of the launch path
+        return torch._C._cuda_getCurrentRawStream(torch.cuda.current_device())
 
     def workspace(self) -> torch.Tensor:
         """Reduction workspace (b2s_ws_bytes), one per (device, stream), zero-filled once."""

@@ -11,9 +11,18 @@ One process, one GPU.
   * Plan build: wall time of plan creation, value coding and template detection (each ends in a host sync), median of 3.
   * Host dispatch: host time per dist_csr_array.dot enqueue at world size 1 (1,000 calls back to back, no sync inside),
     next to the device time per call.
+  * Pipeline sweep: tools/sweep_templates_kernels.cu, compiled into a temporary directory, builds the kernel at every
+    pipeline depth D in {1, 2, 3} and launch bound of 4, 5, 6 or 8 CTAs of 256 threads per SM, at R in {1, 2}; each is
+    timed on fp64 and fp32 L5 (and at R = 1 on the fp64 control) with its registers and spill bytes from ptxas.
+  * Copy ceiling: y.copy_(x) on as many fp64 elements as L5 has rows plus a read of one byte per row -- the traffic
+    of the fp64 template kernel with no gathers and no ids to wait for -- timed like the kernels.
 Moved bytes of the template kernel: one id byte per row, x and y once, the table per CTA (from L2).  The card's name and
 power limit are printed with the numbers.
 """
+import ctypes
+import re
+import subprocess
+import tempfile
 import argparse
 import json
 import os
@@ -30,6 +39,35 @@ from legate.sparse_b200 import dist as bd  # noqa: E402
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 from bench_packed import card, time_per_launch  # noqa: E402
+
+
+def build_sweep_lib(tmp):
+    """The sweep's kernels as a shared object under tmp, and {(value, R, D, MINB): (registers, spill bytes)}."""
+    here = os.path.dirname(os.path.abspath(__file__))
+    so = os.path.join(tmp, "libsweep_templates.so")
+    cmd = ["nvcc", "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-Xcompiler", "-fPIC", "-shared",
+           "-Xptxas", "-v", "-I", os.path.join(os.path.dirname(here), "include"),
+           os.path.join(here, "sweep_templates_kernels.cu"), _lib.lib._name, "-o", so]
+    if os.path.exists("/usr/bin/g++"):
+        cmd[1:1] = ["-ccbin", "/usr/bin/g++"]
+    out = subprocess.run(cmd, capture_output=True, text=True, check=True).stderr
+    regs, cur = {}, None
+    for line in out.splitlines():
+        m = re.search(r"(?:Compiling entry function '|Function properties for )(_Z\w+)", line)
+        if m:
+            k = re.search(r"spmv_template_kernelI([fd])Li5ELi(\d)ELi256ELi(\d)ELi(\d)ELb0E", m.group(1))
+            cur = ("fp64" if k.group(1) == "d" else "fp32",) + tuple(int(g) for g in k.groups()[1:]) if k else None
+            continue
+        if cur is None:
+            continue
+        if (m := re.search(r"(\d+) bytes spill stores", line)):
+            regs.setdefault(cur, [0, 0])[1] = int(m.group(1))
+        if (m := re.search(r"Used (\d+) registers", line)):
+            regs.setdefault(cur, [0, 0])[0] = int(m.group(1))
+    lib = ctypes.CDLL(so)
+    lib.sweep_template_launch.argtypes = [ctypes.c_int] * 4 + [ctypes.c_void_p, ctypes.c_int64, ctypes.c_int] + \
+        [ctypes.c_void_p] * 3
+    return lib, regs
 
 
 def set_shape(rows, threads, streaming):
@@ -71,6 +109,8 @@ def main():
         "l3_1d_fp64": sparse.diags([-1.0, 2.0, -1.0], [-1, 0, 1], shape=(n, n), format="csr", dtype=np.float64),
     }
     shapes = [(r, t, s) for r in (1, 2) for t in (128, 256) for s in (0, 1)]
+    tmp = tempfile.mkdtemp(prefix="sweep_templates_")
+    sweep, regs = build_sweep_lib(tmp)
     cases = {}
     for name, A in mats.items():
         plan = A._get_plan()
@@ -86,6 +126,18 @@ def main():
         for shp in shapes if name != "l3_1d_fp64" else [(0, 0, 0)]:
             cases[f"{name}_tpl_R{shp[0]}_T{shp[1]}_{'cs' if shp[2] else 'st'}"] = dict(
                 run=run, plan=plan, mode=3, shape=shp, moved=moved, flops=2 * A.nnz)
+        vt = name.split("_")[-1]
+        for (v, r, d, m), (nreg, spill) in sorted(regs.items()):
+            if v != vt or (name == "l3_1d_fp64" and r != 1):
+                continue
+
+            def run_pipe(plan=plan, x=x, y=y, A=A, key=(v, r, d, m)):
+                _lib.check(sweep.sweep_template_launch(int(key[0] == "fp64"), key[2], key[3], key[1],
+                                                       plan.tpl_buf.data_ptr(), A.shape[0], 5, x.data_ptr(),
+                                                       y.data_ptr(), torch.cuda.current_stream().cuda_stream),
+                           "sweep_template_launch")
+            cases[f"{name}_pipe_R{r}_D{d}_M{m}"] = dict(run=run_pipe, plan=plan, mode=3, shape=(0, 0, 0), moved=moved,
+                                                        flops=2 * A.nnz, regs=nreg, spill=spill)
         if plan.coded:
             cases[f"{name}_coded"] = dict(run=run, plan=plan, mode=2, shape=(0, 0, 0), moved=None, flops=2 * A.nnz)
 
@@ -113,20 +165,40 @@ def main():
     pt = [time_per_launch(lambda: probe.sum(), 50) for _ in range(3)]
     ceiling = probe.numel() * 8 / float(np.median(pt))
     del probe
+    # copy ceiling of the fp64 L5 template traffic: x read, y written, one byte per row read
+    xc = torch.rand(n, dtype=torch.float64, device="cuda")
+    yc = torch.empty_like(xc)
+    idc = torch.zeros(n // 8, dtype=torch.int64, device="cuda")   # n bytes
+
+    def copy_and_ids():
+        yc.copy_(xc)
+        idc.sum()
+    copy_and_ids()
+    ct = [time_per_launch(copy_and_ids, args.launches) for _ in range(args.reps)]
+    copy_bytes = n * 8 * 2 + idc.numel() * 8
+    copy_ceiling = copy_bytes / float(np.median(ct))
+    del xc, yc, idc
 
     gname, limit = card()
     print(f"# {gname}, power limit {limit} W; {args.launches} launches x {args.reps} alternating rounds per case")
     print(f"# streaming ceiling (probe) {ceiling / 1e12:.3f} TB/s")
+    print(f"# copy ceiling: y.copy_(x) on {n} fp64 + {n} bytes read: {float(np.median(ct)) * 1e6:.1f} us, "
+          f"{copy_bytes / 1e6:.1f} MB, {copy_ceiling / 1e12:.3f} TB/s")
     rows = {}
     for k, c in cases.items():
         ts = sorted(times[k])
         t = float(np.median(ts))
         row = {"us_median": t * 1e6, "us_min": ts[0] * 1e6, "us_max": ts[-1] * 1e6, "gflops": c["flops"] / t / 1e9}
         if c["moved"]:
-            row.update(moved_bytes=c["moved"], moved_tbs=c["moved"] / t / 1e12, moved_frac_of_probe=c["moved"] / t / ceiling)
+            row.update(moved_bytes=c["moved"], moved_tbs=c["moved"] / t / 1e12, moved_frac_of_probe=c["moved"] / t / ceiling,
+                       moved_frac_of_copy=c["moved"] / t / copy_ceiling)
+        if "regs" in c:
+            row.update(registers=c["regs"], spill_bytes=c["spill"])
         rows[k] = row
         mv = f"  moved {c['moved'] / 1e6:6.1f} MB {row['moved_tbs']:.3f} TB/s = {row['moved_frac_of_probe']:.3f} of probe" \
-            if c["moved"] else ""
+             f", {row['moved_frac_of_copy']:.3f} of copy" if c["moved"] else ""
+        if "regs" in c:
+            mv += f"  [{c['regs']} regs, {c['spill']} B spilled]"
         print(f"{k:28s} {t * 1e6:8.1f} us [{ts[0] * 1e6:.1f}..{ts[-1] * 1e6:.1f}]  {row['gflops']:7.1f} GFLOP/s{mv}")
 
     build = {name: plan_build_ms(A) for name, A in mats.items() if name != "l3_1d_fp64"}
@@ -157,7 +229,8 @@ def main():
         os.makedirs(args.out, exist_ok=True)
         with open(os.path.join(args.out, "sweep_templates.json"), "w") as f:
             json.dump({"gpu": gname, "power_limit_w": limit, "launches": args.launches, "reps": args.reps,
-                       "probe_tbs": ceiling / 1e12, "cases": rows, "plan_build_ms": build,
+                       "probe_tbs": ceiling / 1e12,
+                       "copy_ceiling_tbs": copy_ceiling / 1e12, "copy_ceiling_us": float(np.median(ct)) * 1e6, "cases": rows, "plan_build_ms": build,
                        "dot_host_us_per_enqueue": host_us, "dot_device_us_per_call": dev_us}, f, indent=1)
 
 
