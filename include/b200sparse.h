@@ -116,9 +116,10 @@ int         b2s_spmv_plan_info(const void* plan, int64_t* out4_host);
  * Row templates.  The signature of a row is its length, then column - row of each entry in stored order, then the bit
  * patterns of the values.  When every row has at most 8 entries and the matrix has at most 32 distinct signatures
  * (stencils on structured grids: 9 for a 5-point Laplacian, 27 for a 3-D 7-point one), the plan can hold the distinct
- * signatures and one uint8 template id per row; b2s_spmv_csr and b2s_spmv_csr_dot with the same `vals` pointer then
- * read the ids, x and y only, and compute y bit for bit as the other kernels of the plan do.  The tile-range, fused,
- * accumulating and host-vector entry points keep the tile kernels.
+ * signatures, one uint8 template id per row and one uint8 code per group of 32 rows (the template all its rows share,
+ * or 0xFF when they hold more than one); b2s_spmv_csr and b2s_spmv_csr_dot with the same `vals` pointer then read the
+ * codes, the ids of mixed groups only, x and y, and compute y bit for bit as the other kernels of the plan do.  The
+ * tile-range, fused, accumulating and host-vector entry points keep the tile kernels.
  *   b2s_spmv_plan_templates_bytes: size of the DEVICE buffer (16-byte aligned) they need; 0 = the plan cannot use them
  *                                  (only plans whose tiles all take the one-lane-per-row kernel can);
  *   b2s_spmv_plan_templates      : detects the templates (two passes over the matrix, every row compared with its

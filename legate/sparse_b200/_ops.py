@@ -92,8 +92,21 @@ class SpmvPlan:
         tiles = f"b2s::spmv_{'tma' if self.tma else 'tile'}_kernel cfg {self.config} [{fl}]"
         if self.templated:
             # whole-matrix products; tile ranges, fused exchanges and y += A x keep the tile kernel
-            return f"b2s::spmv_template_kernel [{self.ntemplates} row templates, uint8 id per row; tiles: {tiles}]"
+            return f"b2s::spmv_template_kernel [{self.ntemplates} row templates, uint8 code per 32-row group, ids of mixed groups; tiles: {tiles}]"
         return tiles
+
+    # bytes of the TemplateTable at the head of tpl_buf (spmv_common.cuh)
+    TPL_TABLE_BYTES = 32 * 8 * 8 + 32 * 8 + 32 * 8 * 4 + 32 * 4
+
+    def template_sections(self, nrows):
+        """tools / tests: (ids, codes) -- uint8 views of tpl_buf's per-row template ids and per-32-row-group codes
+        (0xFF for a group whose rows hold more than one template)."""
+        r16 = lambda b: (b + 15) // 16 * 16  # noqa: E731
+        ngroups = (nrows + 31) // 32
+        ids_off, codes_off = self.TPL_TABLE_BYTES, self.TPL_TABLE_BYTES + r16(nrows)
+        raw = self.tpl_buf.view(torch.uint8)
+        assert raw.numel() == codes_off + r16(ngroups), (raw.numel(), nrows)
+        return raw[ids_off:ids_off + nrows], raw[codes_off:codes_off + ngroups]
 
     def __del__(self):
         h, self.handle = getattr(self, "handle", None), None
@@ -156,8 +169,8 @@ def spmv_plan_code(plan: SpmvPlan, indptr: torch.Tensor, indices: torch.Tensor, 
 def spmv_plan_templates(plan: SpmvPlan, indptr: torch.Tensor, indices: torch.Tensor, data: torch.Tensor) -> SpmvPlan:
     """Give a plan that no launch has used yet row templates when the matrix qualifies (rows of at most 8 entries, at
     most 32 distinct (length, column - row, value bits) signatures -- structured-grid stencils): whole-matrix products
-    with this `data` then read one uint8 id per row instead of the matrix, so the plan is also only valid while `data`
-    is unchanged.  Otherwise, or for a plan that cannot use them, the plan is returned as it was."""
+    with this `data` then read one uint8 code per 32-row group (and the per-row ids of groups that mix templates)
+    instead of the matrix, so the plan is also only valid while `data` is unchanged.  Otherwise, or for a plan that cannot use them, the plan is returned as it was."""
     if getattr(plan, "handle", None) is None:
         return plan
     nbytes = int(L.b2s_spmv_plan_templates_bytes(plan.handle))

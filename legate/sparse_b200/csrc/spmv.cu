@@ -370,30 +370,40 @@ __global__ void tpl_table_kernel(const P* __restrict__ indptr, const I* __restri
 
 // Pass 2: ids[r] = the template whose hash matches row r's, after comparing the row with it entry by entry; any row
 // that matches no template sets *bad (a hash collision among them included), and the plan then has no templates.
+// Blocks start at multiples of 256 rows, so each warp holds one 32-row group: it votes codes[group] (its rows' common
+// id, or kTplMixed) with every lane, the rows past nrows abstaining.
 template <typename I, typename P>
 __global__ void __launch_bounds__(256)
 tpl_assign_kernel(int64_t nrows, const P* __restrict__ indptr, const I* __restrict__ indices,
                   const void* __restrict__ vals, int vbytes, const TemplateTable* __restrict__ tab, int n,
-                  uint8_t* __restrict__ ids, int* __restrict__ bad) {
+                  uint8_t* __restrict__ ids, uint8_t* __restrict__ codes, int* __restrict__ bad) {
   __shared__ unsigned long long sh[kMaxTemplates];
   if ((int)threadIdx.x < kMaxTemplates) sh[threadIdx.x] = tab->hash[threadIdx.x];
   __syncthreads();
   const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (r >= nrows) return;
-  unsigned long long h = 0;
+  const bool in = r < nrows;
   int t = -1;
-  if (tpl_row_hash(indptr, indices, vals, vbytes, r, &h))
-    for (int i = 0; i < n; i++) t = sh[i] == h ? i : t;
-  bool ok = t >= 0;
-  if (ok) {
-    const long long k0 = (long long)indptr[r];
-    const int len = (int)((long long)indptr[r + 1] - k0);
-    ok = len == tab->len[t];
-    for (int j = 0; ok && j < len; j++)
-      ok = (long long)indices[k0 + j] - r == (long long)tab->off[t][j] && tpl_bits(vals, vbytes, k0 + j) == tab->bits[t][j];
+  if (in) {
+    unsigned long long h = 0;
+    if (tpl_row_hash(indptr, indices, vals, vbytes, r, &h))
+      for (int i = 0; i < n; i++) t = sh[i] == h ? i : t;
+    bool ok = t >= 0;
+    if (ok) {
+      const long long k0 = (long long)indptr[r];
+      const int len = (int)((long long)indptr[r + 1] - k0);
+      ok = len == tab->len[t];
+      for (int j = 0; ok && j < len; j++)
+        ok = (long long)indices[k0 + j] - r == (long long)tab->off[t][j] &&
+             tpl_bits(vals, vbytes, k0 + j) == tab->bits[t][j];
+    }
+    if (!ok) t = 0;
+    ids[r] = (uint8_t)t;
+    if (!ok) atomicExch(bad, 1);
   }
-  ids[r] = (uint8_t)(ok ? t : 0);
-  if (!ok) atomicExch(bad, 1);
+  // lane 0 holds the group's first row, so it is in range whenever any lane is
+  const int first = __shfl_sync(0xffffffffu, t, 0);
+  const bool uniform = __all_sync(0xffffffffu, !in || t == first);
+  if ((threadIdx.x & 31) == 0 && in) codes[r >> 5] = (uint8_t)(uniform ? first : kTplMixed);
 }
 
 // Sections of the packed-structure buffer: tile bases, columns, row offsets, value dictionary (each 16-byte aligned)
@@ -506,6 +516,7 @@ static int plan_templates(PlanHandle* h, const P* indptr, const I* indices, cons
   for (int i = 0; i < n; i++) reps_host[i] = sigs[i].second;
   TemplateTable* tab = (TemplateTable*)buf_dev;
   uint8_t* ids = (uint8_t*)buf_dev + kTplIdsOff;
+  uint8_t* codes = (uint8_t*)buf_dev + tpl_codes_off(nrows);
   int lens[kMaxTemplates + 1] = {0};   // lengths, then the bad flag
   // scratch: the representative rows, then the bad flag
   unsigned char* tmp = nullptr;
@@ -518,7 +529,7 @@ static int plan_templates(PlanHandle* h, const P* indptr, const I* indices, cons
   if (le == cudaSuccess) {
     tpl_table_kernel<I, P><<<1, 32, 0, st>>>(indptr, indices, vals, vbytes, reps, n, tab);
     tpl_assign_kernel<I, P><<<(unsigned)((nrows + 255) / 256), 256, 0, st>>>(nrows, indptr, indices, vals, vbytes, tab, n,
-                                                                             ids, bad);
+                                                                             ids, codes, bad);
     le = cudaGetLastError();
   }
   const int* dev_lens = (const int*)((const unsigned char*)buf_dev + offsetof(TemplateTable, len));
@@ -834,11 +845,12 @@ int64_t b2s_spmv_plan_templates_bytes(const void* plan) {
   const PlanHandle* h = (const PlanHandle*)plan;
   if (!h || h->magic != kPlanMagic || h->flavor != 2 || kCfgs[h->cfg].kind != 1) return 0;
   if (h->nrows <= 0 || h->nnz <= 0 || h->ntiles <= 0 || h->short_tiles != h->ntiles) return 0;
-  return kTplIdsOff + round16(h->nrows);
+  return tpl_buf_bytes(h->nrows);
 }
 
 /* Row templates (TemplateTable): when every row has at most 8 entries and the rows have at most 32 distinct signatures,
- * writes the table and one uint8 id per row into buf_dev (b2s_spmv_plan_templates_bytes bytes, 16-byte aligned,
+ * writes the table, one uint8 id per row and one uint8 code per 32-row group (the group's common id, or kTplMixed),
+ * each section 16-byte aligned, into buf_dev (b2s_spmv_plan_templates_bytes bytes, 16-byte aligned,
  * caller-owned, kept alive and unchanged as long as the plan is used) and switches whole-matrix launches with this
  * `vals` pointer to the template kernel.  Otherwise the plan is left as it was.  Two host syncs. */
 int b2s_spmv_plan_templates(void* plan, const void* indptr, const void* indices, const void* vals, void* buf_dev,
@@ -962,10 +974,11 @@ static int spmv_impl(int vt, int it, int pt, int64_t nrows, int64_t ncols, int64
     TemplateLaunch t;
     t.tab = h->tpl;
     t.ids = (const uint8_t*)h->tpl + kTplIdsOff;
+    t.codes = (const uint8_t*)h->tpl + tpl_codes_off(h->nrows);
     t.nrows = nrows;
     t.maxlen = h->tpl_maxlen;
     const int rows = g_tpl_rows.load(), threads = g_tpl_threads.load();
-    t.rows = rows > 0 ? rows : kTplRowsDefault;
+    t.rows = rows > 0 ? rows : dot ? kTplRowsDefaultDot : kTplRowsDefault;
     t.threads = threads > 0 ? threads : kTplThreadsDefault;
     t.streaming = g_tpl_streaming.load();
     t.x = x; t.y = y;

@@ -134,19 +134,24 @@ constexpr int kPackColGap = 16, kPackRowGap = 8;
 // Row templates (b2s_spmv_plan_templates).  The signature of row r is its length, then indices[k] - r for its entries
 // in stored order, then the bit patterns of their values.  When every row has at most kTplLen entries and the matrix has
 // at most kMaxTemplates distinct signatures (the 9 of a 5-point Laplacian, the 27 of a 3-D 7-point stencil), a plan
-// keeps the signatures in a table and one uint8 template id per row, and a whole-matrix product streams only the ids,
-// x and y.  Templates are sorted by signature hash, so the ids of a matrix do not depend on the run.
+// keeps the signatures in a table, one uint8 template id per row and one uint8 code per group of 32 rows: the template
+// all of the group's rows share, or kTplMixed when they hold more than one.  A whole-matrix product streams the codes,
+// x and y, and the ids of mixed groups only (the rows at a grid-row boundary).  Templates are sorted by signature hash,
+// so the ids of a matrix do not depend on the run.
 constexpr int kMaxTemplates = 32, kTplLen = 8;
+constexpr int kTplMixed = 0xFF;   // a group code that is no template id (ids are below kMaxTemplates)
 struct __align__(16) TemplateTable {
   unsigned long long bits[kMaxTemplates][kTplLen];   // value bit patterns (fp32: the low 32 bits); 0 past the length
   unsigned long long hash[kMaxTemplates];            // signature hashes (ascending; plan time only)
   int off[kMaxTemplates][kTplLen];                   // column - row; 0 past the length
   int len[kMaxTemplates];
 };
-// the template buffer: the table, then ids[nrows]
+// the template buffer: the table, then ids[nrows], then codes[ceil(nrows / 32)], each section 16-byte aligned
 constexpr int64_t kTplIdsOff = (sizeof(TemplateTable) + 15) & ~(size_t)15;
-// default kernel shape: rows per lane, threads per CTA (DESIGN.md 8)
-constexpr int kTplRowsDefault = 1, kTplThreadsDefault = 256;
+inline int64_t tpl_codes_off(int64_t nrows) { return kTplIdsOff + ((nrows + 15) & ~(int64_t)15); }
+inline int64_t tpl_buf_bytes(int64_t nrows) { return tpl_codes_off(nrows) + (((nrows + 31) / 32 + 15) & ~(int64_t)15); }
+// default kernel shape: rows per lane (plain products / the fused dot), threads per CTA (DESIGN.md 8)
+constexpr int kTplRowsDefault = 2, kTplRowsDefaultDot = 1, kTplThreadsDefault = 256;
 
 struct SpmvArgs {
   int64_t ntiles, nrows, nnz;
@@ -178,7 +183,8 @@ int spmv_rowgroup_f64(int it, int pt, int64_t nrows, int64_t nnz, const void* in
 // CTA, streaming = evict-first y stores.  Without dot, w / dot_out / ws are unused.
 struct TemplateLaunch {
   const TemplateTable* tab;
-  const uint8_t* ids;
+  const uint8_t* ids;     // one per row
+  const uint8_t* codes;   // one per 32-row group
   int64_t nrows;
   int maxlen, rows, threads, streaming;
   const void* x;

@@ -911,36 +911,43 @@ spmv_rowgroup_kernel(int64_t nrows, const P* __restrict__ indptr, const I* __res
 
 // ---------------------------------------------------------------------------------------------
 // Row templates (TemplateTable): y[r] = sum_j val[t][j] * x[r + off[t][j]] with t = ids[r].  No matrix stream but one
-// byte per row, so no staging ring either: the table sits in shared memory, a warp takes chunks of 32 R consecutive
-// rows (lane l: rows l + 32 q).  A grid of resident CTAs walks the chunks in row order, so the rows in flight span a
-// few MB of x and its +-n1 neighbours stay in L2.
+// code byte per 32-row group, so no staging ring either: the table sits in shared memory, a warp takes chunks of 32 R
+// consecutive rows (lane l: rows l + 32 q, group R c + q).  A grid of resident CTAs walks the chunks in row order, so
+// the rows in flight span a few MB of x and its +-n1 neighbours stay in L2.
+// A group's code is its rows' common template, read by the whole warp from one address; only a mixed group (kTplMixed:
+// on a structured grid, one holding a grid-row boundary, about 1 % of them) reads its rows' ids, just before its
+// gathers.  On a uniform group every lane indexes the same template, so the table reads are broadcasts.
 // Software pipeline of depth D over each warp's chunks c_i = c_0 + i S (S = gridDim.x * warps per CTA): while chunk i
-// is summed and stored, the x gathers of chunks i+1 .. i+D-1 and the ids of chunks up to i+D+1 are already in flight.
-// Without it a chunk costs two dependent memory trips (its ids, then its gathers) with nothing else outstanding in the
-// warp.  The ids of a chunk are loaded two steps before its gathers, its gathers D-1 steps before its sum.  Chunks
-// past the end load nothing (their rows are all >= nrows).  Both rings are indexed by compile-time slots of a loop
-// unrolled NT times, so no value moves between registers while its load is still pending.
+// is summed and stored, the x gathers of chunks i+1 .. i+D-1 and the codes of chunks up to i+D+1 are already in
+// flight.  Without it a chunk costs two dependent memory trips (its code, then its gathers) with nothing else
+// outstanding in the warp.  The codes of a chunk are loaded two steps before its gathers, its gathers D-1 steps before
+// its sum.  Chunks past the end load nothing (their rows are all >= nrows).  The rings are indexed by compile-time
+// slots of a loop unrolled NT times, so no value moves between registers while its load is still pending.
 // Each sum is formed exactly as the one-lane-per-row CSR path forms it (short_row_sum: U terms from +0 in stored order,
 // zero products past the row's end, then + 0.0 in place of the old y), so y is bit-identical to the other kernels of
 // the same plan -- up to which NaN survives where two different NaNs meet in one FMA (an inf - inf sum times a NaN in
 // x), which follows the operand order the compiler picked for that FMA.
 // ---------------------------------------------------------------------------------------------
+// The codes of chunk c, groups R c .. R c + R - 1, in the low R bytes (one 8- or 16-bit load: the codes section is
+// 16-byte aligned); groups past the end read as 0
 template <int R>
-__device__ __forceinline__ void tpl_load_ids(int (&t)[R], const uint8_t* __restrict__ ids, int64_t c, int64_t nrows,
-                                             int lane) {
-#pragma unroll
-  for (int q = 0; q < R; q++) {
-    const int64_t r = c * (32 * R) + 32 * q + lane;
-    t[q] = r < nrows ? (int)__ldcs(ids + r) : 0;
-  }
+__device__ __forceinline__ int tpl_load_codes(const uint8_t* __restrict__ codes, int64_t c, int64_t ngroups) {
+  static_assert(R == 1 || R == 2, "one or two rows per lane");
+  const int64_t g0 = c * R;
+  if (R == 2 && g0 + 1 < ngroups) return (int)__ldg(reinterpret_cast<const unsigned short*>(codes + g0));
+  return g0 < ngroups ? (int)__ldg(codes + g0) : 0;
 }
 
+// t[q]: the template of this lane's row q of chunk c, from the chunk's codes g (the row's id in a mixed group)
 template <typename V, int U, int R>
-__device__ __forceinline__ void tpl_gather(V (&xv)[R][U], const int (&t)[R], const int (*soff)[U], const int* slen,
-                                           const V* __restrict__ x, int64_t c, int64_t nrows, int lane) {
+__device__ __forceinline__ void tpl_gather(V (&xv)[R][U], int (&t)[R], int g, const uint8_t* __restrict__ ids,
+                                           const int (*soff)[U], const int* slen, const V* __restrict__ x, int64_t c,
+                                           int64_t nrows, int lane) {
 #pragma unroll
   for (int q = 0; q < R; q++) {
     const int64_t r = c * (32 * R) + 32 * q + lane;
+    t[q] = (g >> (8 * q)) & 0xFF;
+    if (t[q] == kTplMixed) t[q] = r < nrows ? (int)__ldcs(ids + r) : 0;
     const int n = r < nrows ? slen[t[q]] : 0;
 #pragma unroll
     for (int j = 0; j < U; j++) xv[q][j] = j < n ? __ldg(x + (r + soff[t[q]][j])) : (V)0;
@@ -948,11 +955,12 @@ __device__ __forceinline__ void tpl_gather(V (&xv)[R][U], const int (&t)[R], con
 }
 
 // Pipeline depth D (chunks whose gathers are in flight, the one being summed included) and CTAs of 256 threads per SM
-// the launch bound asks for: the sweep in DESIGN.md 8 (tools/sweep_templates.py).  On an H100 at 700 W, loading the ids
-// ahead (D = 1) was fastest for fp64 and fp32, with and without the fused dot; deeper rings gained nothing once fp64 L5
-// ran at the copy ceiling, and cost occupancy (the fp64 dot: 168-170 us against 153 on pde.py's operator).  No bound
-// spills: fp64 products of rows of up to 5 entries keep the 32 registers of 8 CTAs (the fastest), the fused dot 46-48 (5
-// CTAs; 8 CTAs lose 1.5 %), the rest 40 (6 CTAs), and two rows per lane 48 or, with the fp64 dot, 64 (4 CTAs).
+// the launch bound asks for: the sweep in DESIGN.md 8 (tools/sweep_templates.py).  On an H100 at 700 W, loading each
+// chunk's codes ahead of its gathers (D = 1) was fastest for fp64 and fp32, with and without the fused dot; deeper
+// rings gained nothing once fp64 L5 ran at the copy ceiling, and cost occupancy (the fp64 dot: 168-170 us against 153
+// on pde.py's operator).  No bound spills: at one row per lane, fp64 products of rows of up to 5 entries keep the 32
+// registers of 8 CTAs, the fused dot 45-48 (5 CTAs; 8 CTAs lose 1.5 %), the rest 40 (6 CTAs); two rows per lane (the
+// default for plain products) 46-48 (5 CTAs) or, with the fp64 dot, 58 (4 CTAs).
 template <typename V, int U, int R, bool DOT> struct TplPipe {
   static constexpr int D = 1;
   static constexpr int MINB = R == 2 ? (DOT && sizeof(V) == 8 ? 4 : 5) : DOT ? 5 : (U == 5 && sizeof(V) == 8 ? 8 : 6);
@@ -960,9 +968,9 @@ template <typename V, int U, int R, bool DOT> struct TplPipe {
 
 template <typename V, int U, int R, int THREADS, int D, int MINB, bool DOT>
 __global__ void __launch_bounds__(THREADS, MINB)
-spmv_template_kernel(int64_t nrows, const uint8_t* __restrict__ ids, const TemplateTable* __restrict__ tab,
-                     const V* __restrict__ x, V* __restrict__ y, int streaming, const V* __restrict__ w, V* dot_out,
-                     void* ws) {
+spmv_template_kernel(int64_t nrows, const uint8_t* __restrict__ ids, const uint8_t* __restrict__ codes,
+                     const TemplateTable* __restrict__ tab, const V* __restrict__ x, V* __restrict__ y, int streaming,
+                     const V* __restrict__ w, V* dot_out, void* ws) {
   static_assert(D >= 1 && D <= 3, "pipeline depth 1..3");
   __shared__ int soff[kMaxTemplates][U];
   __shared__ V sval[kMaxTemplates][U];
@@ -979,26 +987,31 @@ spmv_template_kernel(int64_t nrows, const uint8_t* __restrict__ ids, const Templ
   if (threadIdx.x < kMaxTemplates) slen[threadIdx.x] = tab->len[threadIdx.x];
   __syncthreads();
   constexpr int WPB = THREADS / 32;
-  // id ring: chunks i .. i+D+1 are live at step i; a multiple of D so that one unrolled pass returns both rings to slot 0
+  // code ring: chunks i .. i+D+1 are live at step i; a multiple of D so that one unrolled pass returns both rings to
+  // slot 0
   constexpr int NT = D * ((D + 2 + D - 1) / D);
   const int lane = threadIdx.x & 31;
   const int64_t nchunks = (nrows + 32 * R - 1) / (32 * R);
+  const int64_t ngroups = (nrows + 31) / 32;
   const int64_t S = (int64_t)gridDim.x * WPB;
   int64_t c = (int64_t)blockIdx.x * WPB + (threadIdx.x >> 5);
-  int t[NT][R];
+  int g[NT];
+  int t[D][R];
   V xv[D][R][U];
 #pragma unroll
-  for (int k = 0; k <= D; k++) tpl_load_ids<R>(t[k], ids, c + k * S, nrows, lane);
+  for (int k = 0; k <= D; k++) g[k] = tpl_load_codes<R>(codes, c + k * S, ngroups);
 #pragma unroll
-  for (int k = 0; k < D - 1; k++) tpl_gather<V, U, R>(xv[k], t[k], soff, slen, x, c + k * S, nrows, lane);
+  for (int k = 0; k < D - 1; k++)
+    tpl_gather<V, U, R>(xv[k], t[k], g[k], ids, soff, slen, x, c + k * S, nrows, lane);
   double dot_acc = 0.0;
   while (c < nchunks) {
 #pragma unroll
     for (int k = 0; k < NT; k++) {
       if (c >= nchunks) break;
-      tpl_gather<V, U, R>(xv[(k + D - 1) % D], t[(k + D - 1) % NT], soff, slen, x, c + (D - 1) * S, nrows, lane);
-      tpl_load_ids<R>(t[(k + D + 1) % NT], ids, c + (D + 1) * S, nrows, lane);
-      const int (&tc)[R] = t[k % NT];
+      tpl_gather<V, U, R>(xv[(k + D - 1) % D], t[(k + D - 1) % D], g[(k + D - 1) % NT], ids, soff, slen, x,
+                          c + (D - 1) * S, nrows, lane);
+      g[(k + D + 1) % NT] = tpl_load_codes<R>(codes, c + (D + 1) * S, ngroups);
+      const int (&tc)[R] = t[k % D];
       const V (&xc)[R][U] = xv[k % D];
 #pragma unroll
       for (int q = 0; q < R; q++) {
@@ -1215,7 +1228,7 @@ static int launch_template_f(const TemplateLaunch& a) {
   if (DOT && grid > WS_MAX_PARTIALS) grid = WS_MAX_PARTIALS;
   if (grid > want) grid = want;
   if (grid < 1) grid = 1;
-  kern<<<(unsigned)grid, THREADS, 0, a.st>>>(a.nrows, a.ids, a.tab, (const V*)a.x, (V*)a.y, a.streaming,
+  kern<<<(unsigned)grid, THREADS, 0, a.st>>>(a.nrows, a.ids, a.codes, a.tab, (const V*)a.x, (V*)a.y, a.streaming,
                                              (const V*)a.w, (V*)a.dot_out, a.ws);
   B2S_LAUNCH_CHECK();
   return B2S_OK;

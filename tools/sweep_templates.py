@@ -14,10 +14,14 @@ One process, one GPU.
   * Pipeline sweep: tools/sweep_templates_kernels.cu, compiled into a temporary directory, builds the kernel at every
     pipeline depth D in {1, 2, 3} and launch bound of 4, 5, 6 or 8 CTAs of 256 threads per SM, at R in {1, 2}; each is
     timed on fp64 and fp32 L5 (and at R = 1 on the fp64 control) with its registers and spill bytes from ptxas.
-  * Copy ceiling: y.copy_(x) on as many fp64 elements as L5 has rows plus a read of one byte per row -- the traffic
-    of the fp64 template kernel with no gathers and no ids to wait for -- timed like the kernels.
-Moved bytes of the template kernel: one id byte per row, x and y once, the table per CTA (from L2).  The card's name and
-power limit are printed with the numbers.
+  * Copy ceiling: y.copy_(x) on as many fp64 elements as L5 has rows plus a read of one byte per row (two torch
+    launches), timed like the kernels.
+  * Native ceiling: one launch of a streaming kernel on the template kernel's grid (one resident wave of 256-thread CTAs,
+    32-element chunks per warp) that copies as many fp64 elements as L5 has rows and reads m more bytes: at m = nrows
+    (one id per row) and at m = the fp64 L5 plan's code and mixed-group id bytes -- the template kernel's traffic with no
+    gathers and nothing to wait for.
+Moved bytes of the template kernel: one code byte per 32-row group, 32 id bytes per mixed group, x and y once, the
+table per CTA (from L2).  The card's name and power limit are printed with the numbers.
 """
 import ctypes
 import re
@@ -67,6 +71,8 @@ def build_sweep_lib(tmp):
     lib = ctypes.CDLL(so)
     lib.sweep_template_launch.argtypes = [ctypes.c_int] * 4 + [ctypes.c_void_p, ctypes.c_int64, ctypes.c_int] + \
         [ctypes.c_void_p] * 3
+    lib.sweep_stream_ceiling.argtypes = [ctypes.c_int64, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p,
+                                         ctypes.c_int64, ctypes.c_void_p, ctypes.c_void_p]
     return lib, regs
 
 
@@ -112,6 +118,7 @@ def main():
     tmp = tempfile.mkdtemp(prefix="sweep_templates_")
     sweep, regs = build_sweep_lib(tmp)
     cases = {}
+    id_bytes = {}
     for name, A in mats.items():
         plan = A._get_plan()
         assert plan.templated, (name, plan.kernel_name)
@@ -122,7 +129,10 @@ def main():
             _ops.spmv(A.indptr, A.indices, A.data, x, y, A.shape, plan=plan)
 
         sv = A.data.element_size()
-        moved = A.shape[0] + A.shape[0] * sv + A.shape[1] * sv
+        _, codes = plan.template_sections(A.shape[0])
+        mixed = int((codes == 0xFF).sum())
+        id_bytes[name] = dict(groups=codes.numel(), mixed=mixed, bytes=codes.numel() + 32 * mixed)
+        moved = id_bytes[name]["bytes"] + A.shape[0] * sv + A.shape[1] * sv
         for shp in shapes if name != "l3_1d_fp64" else [(0, 0, 0)]:
             cases[f"{name}_tpl_R{shp[0]}_T{shp[1]}_{'cs' if shp[2] else 'st'}"] = dict(
                 run=run, plan=plan, mode=3, shape=shp, moved=moved, flops=2 * A.nnz)
@@ -177,6 +187,21 @@ def main():
     ct = [time_per_launch(copy_and_ids, args.launches) for _ in range(args.reps)]
     copy_bytes = n * 8 * 2 + idc.numel() * 8
     copy_ceiling = copy_bytes / float(np.median(ct))
+    # the native ceiling, one launch on the template kernel's grid, at the parent's and this kernel's id traffic
+    sink = torch.zeros(4, dtype=torch.int32, device="cuda")
+    native = {}
+    for label, m in (("one id per row", n), ("group codes", id_bytes["l5_fp64"]["bytes"])):
+        mb = torch.zeros((m + 15) // 16 * 16, dtype=torch.uint8, device="cuda")
+
+        def stream(mb=mb):
+            _lib.check(sweep.sweep_stream_ceiling(n, xc.data_ptr(), yc.data_ptr(), mb.data_ptr(), mb.numel(),
+                                                  sink.data_ptr(), torch.cuda.current_stream().cuda_stream),
+                       "sweep_stream_ceiling")
+        stream()
+        nt = float(np.median([time_per_launch(stream, args.launches) for _ in range(args.reps)]))
+        native[label] = dict(m_bytes=mb.numel(), us=nt * 1e6, moved_bytes=n * 16 + mb.numel(),
+                             tbs=(n * 16 + mb.numel()) / nt / 1e12)
+        del mb
     del xc, yc, idc
 
     gname, limit = card()
@@ -184,6 +209,13 @@ def main():
     print(f"# streaming ceiling (probe) {ceiling / 1e12:.3f} TB/s")
     print(f"# copy ceiling: y.copy_(x) on {n} fp64 + {n} bytes read: {float(np.median(ct)) * 1e6:.1f} us, "
           f"{copy_bytes / 1e6:.1f} MB, {copy_ceiling / 1e12:.3f} TB/s")
+    for label, v in native.items():
+        print(f"# native ceiling ({label}): copy of {n} fp64 + {v['m_bytes'] / 1e6:.2f} MB read, one launch: "
+              f"{v['us']:.1f} us, {v['moved_bytes'] / 1e6:.1f} MB, {v['tbs']:.3f} TB/s")
+    for name, v in id_bytes.items():
+        print(f"# {name}: {v['groups']} groups, {v['mixed']} mixed ({100 * v['mixed'] / v['groups']:.2f} %), "
+              f"{v['bytes'] / 1e6:.2f} MB of codes and ids")
+    native_tbs = native["group codes"]["tbs"] * 1e12
     rows = {}
     for k, c in cases.items():
         ts = sorted(times[k])
@@ -191,12 +223,13 @@ def main():
         row = {"us_median": t * 1e6, "us_min": ts[0] * 1e6, "us_max": ts[-1] * 1e6, "gflops": c["flops"] / t / 1e9}
         if c["moved"]:
             row.update(moved_bytes=c["moved"], moved_tbs=c["moved"] / t / 1e12, moved_frac_of_probe=c["moved"] / t / ceiling,
-                       moved_frac_of_copy=c["moved"] / t / copy_ceiling)
+                       moved_frac_of_copy=c["moved"] / t / copy_ceiling, moved_frac_of_native=c["moved"] / t / native_tbs)
         if "regs" in c:
             row.update(registers=c["regs"], spill_bytes=c["spill"])
         rows[k] = row
         mv = f"  moved {c['moved'] / 1e6:6.1f} MB {row['moved_tbs']:.3f} TB/s = {row['moved_frac_of_probe']:.3f} of probe" \
-             f", {row['moved_frac_of_copy']:.3f} of copy" if c["moved"] else ""
+             f", {row['moved_frac_of_copy']:.3f} of copy, {row['moved_frac_of_native']:.3f} of native" \
+            if c["moved"] else ""
         if "regs" in c:
             mv += f"  [{c['regs']} regs, {c['spill']} B spilled]"
         print(f"{k:28s} {t * 1e6:8.1f} us [{ts[0] * 1e6:.1f}..{ts[-1] * 1e6:.1f}]  {row['gflops']:7.1f} GFLOP/s{mv}")
@@ -230,7 +263,8 @@ def main():
         with open(os.path.join(args.out, "sweep_templates.json"), "w") as f:
             json.dump({"gpu": gname, "power_limit_w": limit, "launches": args.launches, "reps": args.reps,
                        "probe_tbs": ceiling / 1e12,
-                       "copy_ceiling_tbs": copy_ceiling / 1e12, "copy_ceiling_us": float(np.median(ct)) * 1e6, "cases": rows, "plan_build_ms": build,
+                       "copy_ceiling_tbs": copy_ceiling / 1e12, "copy_ceiling_us": float(np.median(ct)) * 1e6,
+                       "native_ceiling": native, "template_id_bytes": id_bytes, "cases": rows, "plan_build_ms": build,
                        "dot_host_us_per_enqueue": host_us, "dot_device_us_per_call": dev_us}, f, indent=1)
 
 
