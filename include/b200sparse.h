@@ -337,7 +337,9 @@ int         b2s_copy(int vt, int64_t n, void* dst, const void* src, void* stream
  * sorted_coords_to_counts.cu:32, nnz_to_pos base.py:30-48) and its CSR->CSC->transpose route (sparse/csr.py:404-424)
  * with a counting sort by row (L2 atomics), a scan and a per-row bitonic sort by column: no global sort.  Unique
  * (row, col) pairs assumed, as in the reference (coo.py:73-76).  `scratch`: b2s_convert_scratch_bytes(nbuckets, pt)
- * bytes with nbuckets = nrows of the OUTPUT matrix.  Both calls sync the stream once. */
+ * bytes with nbuckets = nrows of the OUTPUT matrix.  Both calls sync the stream once.  Values are moved bit for bit,
+ * never combined or converted (no flush of denormals): callers move other 4- or 8-byte payloads through them, as
+ * sparse.random's complex CSC path moves int64 entry positions as float64 bit patterns. */
 int64_t     b2s_convert_scratch_bytes(int64_t nbuckets, int pt);
 int         b2s_coo_to_csr(int vt, int it, int pt, int64_t nrows, int64_t nnz, const void* rows, const void* cols,
                            const void* vals, void* indptr, void* indices, void* vals_out, void* scratch,
@@ -554,6 +556,32 @@ int         b2s_dia_to_csr(int vt, int it, int pt, int64_t nrows, int64_t ncols,
 int         b2s_csr_to_dia(int vt, int it, int pt, int64_t nrows, int64_t ncols, int64_t nnz, const void* indptr,
                            const void* indices, const void* vals, int64_t ndiag, int64_t L, int64_t* offsets,
                            void* data, void* scratch, int64_t scratch_bytes, int64_t* ndiag_L_host, void* stream);
+
+/* ---- random sparse matrices: sparse.random / rand / random_array (csrc/random.cu) --------------------------------
+ * A uniform random k-subset of the nrows x ncols positions and its values, from one 64-bit seed.  The caller samples
+ * s = min(k, mn - k) positions (mn = nrows * ncols): the entries themselves, or the zeros when k > mn - k.
+ *   b2s_random_sample     : s distinct positions, as (rows, cols) of index width `it`, in no particular order.  Draw i
+ *                           of round r, attempt a, is word 0 of the Philox4x64-10 block at key (seed, 0) and counter
+ *                           (i, r, a, 0), mapped onto [0, mn) by Lemire's multiply-high with rejection (a rejected
+ *                           draw retries with a + 1); position p is (p / ncols, p mod ncols).  Round r draws the
+ *                           shortfall s - have and inserts it into `table` (b2s_random_table_slots(s) int64 slots, a
+ *                           power of two >= 2s); positions new to the table are appended to rows / cols.  `counters`:
+ *                           16 bytes of device scratch.  Syncs the stream once per round and writes the number of
+ *                           rounds to *rounds_host.  The set -- not the order of rows / cols -- depends on the seed
+ *                           alone.  Needs s <= mn - s; B2S_ENOMEM if a probe finds the table full.
+ *   b2s_random_complement : the canonical CSR (nnz = mn - z entries) of the positions NOT in the canonical CSR
+ *                           (zptr int64, zidx of width `it`, z entries) of a sampled zero set: indptr[i] =
+ *                           i * ncols - zptr[i], each row's columns ascending.  No sync, no allocation.
+ *   b2s_random_values     : vals[j] for j < nnz from the Philox4x64-10 block at key (seed, 1), counter (j, 0, 0, 0):
+ *                           float64 (w0 >> 11) * 2^-53, float32 (w0 >> 40) * 2^-24, uniform on [0, 1); with
+ *                           is_complex the imaginary part, from w1, follows each real part.  No sync. */
+int64_t     b2s_random_table_slots(int64_t s);
+int         b2s_random_sample(int it, int64_t nrows, int64_t ncols, int64_t s, uint64_t seed, void* table,
+                              int64_t slots, void* rows, void* cols, void* counters, int64_t* rounds_host,
+                              void* stream);
+int         b2s_random_complement(int it, int pt, int64_t nrows, int64_t ncols, int64_t nnz, const int64_t* zptr,
+                                  const void* zidx, void* indptr, void* indices, void* stream);
+int         b2s_random_values(int vt, int is_complex, int64_t nnz, uint64_t seed, void* vals, void* stream);
 
 /* ---- multi-GPU: NCCL communicator owned by the library (SURVEY 8b) -----------------------------------------
  * For hosts without torch.distributed (and for multi-node runs): the library binds NCCL at run time (dlopen of

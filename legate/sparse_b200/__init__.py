@@ -11,7 +11,8 @@ from .csc import csc_array, csc_matrix  # noqa: F401
 from .csr import csr_array, csr_matrix, spgemm_csr_csr_csr  # noqa: F401
 from .dia import dia_array, dia_matrix  # noqa: F401
 from .module import (  # noqa: F401
-    block_diag, bmat, diags, eye, hstack, identity, is_sparse_matrix, kron, kronsum, spdiags, vstack,
+    block_diag, bmat, diags, eye, hstack, identity, is_sparse_matrix, kron, kronsum, rand, random, random_array,
+    spdiags, vstack,
 )
 from .runtime import runtime  # noqa: F401
 from . import io, linalg  # noqa: F401

@@ -15,7 +15,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB_NAME = "libb200sparse.so"
 LIB_PATH = os.path.join(HERE, LIB_NAME)
-SOURCES = ["capi.cu", "spmv.cu", "spmv_f32.cu", "spmv_f64.cu", "spmm.cu", "spmm_tma.cu", "vecops.cu", "spgemm.cu", "peer.cu", "probe.cu", "comm.cu", "convert.cu", "elementwise.cu", "sddmm.cu", "tropical.cu", "reduce.cu", "index.cu", "construct.cu", "csc.cu", "dia.cu"]
+SOURCES = ["capi.cu", "spmv.cu", "spmv_f32.cu", "spmv_f64.cu", "spmm.cu", "spmm_tma.cu", "vecops.cu", "spgemm.cu", "peer.cu", "probe.cu", "comm.cu", "convert.cu", "elementwise.cu", "sddmm.cu", "tropical.cu", "reduce.cu", "index.cu", "construct.cu", "csc.cu", "dia.cu", "random.cu"]
 HEADERS = ["common.cuh", "scan.cuh", "spmv_common.cuh", "spmv_kernels.cuh", os.path.join("..", "..", "..", "include", "b200sparse.h")]
 
 NVCC_FLAGS = [

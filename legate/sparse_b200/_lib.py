@@ -115,6 +115,11 @@ SIGNATURES = {
                                c_vp, c_vp, c_i64, c_vp, c_vp]),
     "b2s_csr_to_dia": (c_i32, [c_i32, c_i32, c_i32, c_i64, c_i64, c_i64, c_vp, c_vp, c_vp, c_i64, c_i64, c_vp, c_vp,
                                c_vp, c_i64, c_vp, c_vp]),
+    "b2s_random_table_slots": (c_i64, [c_i64]),
+    "b2s_random_sample": (c_i32, [c_i32, c_i64, c_i64, c_i64, ctypes.c_uint64, c_vp, c_i64, c_vp, c_vp, c_vp,
+                                  ctypes.POINTER(c_i64), c_vp]),
+    "b2s_random_complement": (c_i32, [c_i32, c_i32, c_i64, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "b2s_random_values": (c_i32, [c_i32, c_i32, c_i64, ctypes.c_uint64, c_vp, c_vp]),
     "b2s_comm_nccl_version": (c_i32, []),
     "b2s_comm_unique_id": (c_i32, [c_vp]),
     "b2s_comm_init": (c_i32, [c_i32, c_i32, c_vp, ctypes.POINTER(c_vp)]),

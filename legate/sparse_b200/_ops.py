@@ -13,7 +13,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from .runtime import idx_code, ptr, runtime, vt_code
+from .runtime import idx_code, ptr, runtime, torch_dtype, vt_code
 
 L = _lib.lib
 
@@ -726,6 +726,63 @@ def csr_blocks(blocks, shape, nnz: int, dtype, out_index_dtype):
                                 table.ctypes.data, ptr(out_ptr), ptr(out_idx), ptr(out_val), ptr(scratch), _stream()),
                "b2s_csr_blocks")
     return out_ptr, out_idx, out_val
+
+
+def random_csr(shape, k: int, seed: int, idx_dtype, ptr_dtype, dtype, data=None):
+    """The canonical CSR arrays (indptr, indices, data) of a uniform random k-subset of the m x n positions, and the
+    number of sampling rounds, through csrc/random.cu: b2s_random_sample of s = min(k, mn - k) positions,
+    b2s_coo_to_csr of them and, when k > mn - k, b2s_random_complement of that zero set.  The values are
+    b2s_random_values of `seed` in `dtype` (float32, float64, complex64 or complex128), or `data`, a device tensor of k
+    values already in canonical order.  Every buffer is allocated before the first launch, so a sample that does not
+    fit raises MemoryError (or torch's out-of-memory error) instead of failing in a kernel.  The sampler syncs once per
+    round, the assembly once."""
+    m, n = shape
+    mn = m * n
+    complement = k > mn - k
+    s = mn - k if complement else k
+    dev = runtime.device
+    slots = int(L.b2s_random_table_slots(s))
+    sptr_dtype = torch.int64 if complement else ptr_dtype   # the zero set's row pointers feed the complement kernel
+    tdt = torch_dtype(dtype)
+    isz, psz, vsz = (torch.empty(0, dtype=t).element_size() for t in (idx_dtype, sptr_dtype, tdt))
+    need = 8 * slots + 3 * s * isz + (m + 1) * psz + int(L.b2s_convert_scratch_bytes(m, idx_code(sptr_dtype)))
+    need += (8 * (m + 1) + k * isz if complement else 0) + (k * vsz if data is None else 0)
+    # free device memory plus what torch's caching allocator holds unused, which it hands out before asking CUDA
+    free = torch.cuda.mem_get_info(dev)[0] + torch.cuda.memory_reserved(dev) - torch.cuda.memory_allocated(dev)
+    if slots == 0 or need > free:
+        raise MemoryError(f"a random {m} x {n} matrix with {k} stored entries needs {need} bytes of device memory to "
+                          f"sample; {free} are free")
+    table = torch.empty(slots, dtype=torch.int64, device=dev)
+    rows, cols = (torch.empty(s, dtype=idx_dtype, device=dev) for _ in range(2))
+    counters = torch.empty(2, dtype=torch.int64, device=dev)
+    sptr = torch.empty(m + 1, dtype=sptr_dtype, device=dev)
+    sidx = torch.empty(s, dtype=idx_dtype, device=dev)
+    scratch = torch.empty(int(L.b2s_convert_scratch_bytes(m, idx_code(sptr_dtype))), dtype=torch.uint8, device=dev)
+    if complement:
+        indptr, indices = torch.empty(m + 1, dtype=ptr_dtype, device=dev), torch.empty(k, dtype=idx_dtype, device=dev)
+    else:
+        indptr, indices = sptr, sidx
+    generate = data is None
+    if generate:
+        data = torch.empty(k, dtype=tdt, device=dev)
+    # b2s_coo_to_csr moves a value per triplet; nothing reads them here, so they live in the table, which is no longer
+    # needed once the sample is drawn (slots >= 2s: room for two float32 arrays of s)
+    moved = table.view(torch.float32)
+    it, st = idx_code(idx_dtype), _stream()
+    rounds = _lib.c_i64(0)
+    _lib.check(L.b2s_random_sample(it, m, n, s, seed, ptr(table), slots, ptr(rows), ptr(cols), ptr(counters),
+                                   ctypes.byref(rounds), st), "b2s_random_sample")
+    bad = _lib.c_i64(0)
+    _lib.check(L.b2s_coo_to_csr(_lib.F32, it, idx_code(sptr_dtype), m, s, ptr(rows), ptr(cols), ptr(moved[:s]),
+                                ptr(sptr), ptr(sidx), ptr(moved[s:2 * s]), ptr(scratch), ctypes.byref(bad), st),
+               "b2s_coo_to_csr")
+    if complement:
+        _lib.check(L.b2s_random_complement(it, idx_code(ptr_dtype), m, n, k, ptr(sptr), ptr(sidx), ptr(indptr),
+                                           ptr(indices), st), "b2s_random_complement")
+    if generate:
+        vt = _lib.F32 if tdt in (torch.float32, torch.complex64) else _lib.F64
+        _lib.check(L.b2s_random_values(vt, int(tdt.is_complex), k, seed, ptr(data), st), "b2s_random_values")
+    return indptr, indices, data, int(rounds.value)
 
 
 def spgemm_row_work(a_indptr, a_indices, b_indptr) -> torch.Tensor:

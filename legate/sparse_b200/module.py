@@ -11,9 +11,13 @@ They keep every stored entry -- stored order, explicit zeros, repeated columns -
 which adds its two Kronecker products with the sparse add (a sum that cancels to zero stays stored).  Unlike scipy,
 which returns BSR or COO by default, they return a `csr_array` for `format=None` and `"csr"`, and `result.tocoo()` for
 `"coo"`; this library has no BSR type and no COO compute path, and other formats raise NotImplementedError.
+
+`random`, `rand` and `random_array` sample uniform random sparse matrices on the device (csrc/random.cu, DESIGN section
+3.16) from one 64-bit seed drawn from the caller's generator.
 """
 from __future__ import annotations
 
+import functools
 import numbers
 from itertools import accumulate
 
@@ -322,3 +326,117 @@ def block_diag(mats, format=None, dtype=None):
     if not placed:
         raise ValueError("need at least one array to concatenate")
     return _assemble(placed, (r, c), _result_dtype([A for *_, A in placed], dtype), format, "block_diag")
+
+
+# ---- random sparse matrices (csrc/random.cu) --------------------------------------------------------------------------
+_RANDOM_DTYPES = tuple(np.dtype(t) for t in (np.float32, np.float64, np.complex64, np.complex128))
+
+
+def _check_random_state(seed):
+    """scipy's check_random_state: None -> numpy's global RandomState, an int -> a new RandomState, a Generator or
+    RandomState as it is."""
+    if seed is None or seed is np.random:
+        return np.random.mtrand._rand
+    if isinstance(seed, (numbers.Integral, np.integer)):
+        return np.random.RandomState(seed)
+    if isinstance(seed, (np.random.RandomState, np.random.Generator)):
+        return seed
+    raise ValueError(f"'{seed}' cannot be used to seed a numpy.random.RandomState instance")
+
+
+def _scipy_rng(position=None):
+    """Resolve `rng` / `random_state` into one generator as scipy 1.18.1 does (its _transition_to_rng): a keyword `rng`
+    through numpy.random.default_rng, a `random_state` keyword or the argument at `position` as check_random_state
+    reads it; the resolved generator reaches the function as `rng`."""
+    def decorate(fun):
+        @functools.wraps(fun)
+        def wrapper(*args, **kwargs):
+            positional = position is not None and len(args) > position
+            if ("random_state" in kwargs) + ("rng" in kwargs) + positional > 1:
+                raise TypeError(f"{fun.__name__}() got multiple values for argument now known as `rng`. Specify one of "
+                                "`rng` or `random_state`.")
+            if "rng" in kwargs:
+                kwargs["rng"] = np.random.default_rng(kwargs["rng"])
+            elif positional:
+                args = (*args[:position], _check_random_state(args[position]), *args[position + 1:])
+            else:
+                kwargs["rng"] = _check_random_state(kwargs.pop("random_state", None))
+            return fun(*args, **kwargs)
+        return wrapper
+    return decorate
+
+
+def _random(shape, density, format, dtype, rng, data_sampler, what):
+    """The one implementation of random, rand and random_array.  Checks as scipy does, draws one 64-bit seed from `rng`,
+    calls `data_sampler(size=k)` once if given, then samples and assembles on the device (`_ops.random_csr`)."""
+    if not 0 <= density <= 1:
+        raise ValueError("density expected to be 0 <= density <= 1")
+    if len(shape) != 2:
+        raise NotImplementedError(f"{what}: a {len(shape)}-D shape; only 2-D random matrices are implemented")
+    m, n = (int(s) for s in shape)
+    if m < 0 or n < 0:
+        raise ValueError("'shape' elements cannot be negative")
+    mn = m * n
+    if mn > _INT64_MAX:
+        raise NotImplementedError(f"{what}: {m} x {n} positions do not fit in int64")
+    k = int(round(density * mn))
+    if format not in ("coo", "csr", "csc", "dia"):
+        raise NotImplementedError(f"{what}(format={format!r}): 'coo', 'csr', 'csc' and 'dia' are implemented")
+    dtype = np.dtype(np.float64 if dtype is None else dtype)
+    if dtype not in _RANDOM_DTYPES:
+        raise NotImplementedError(f"{what} for dtype {dtype} is not implemented (float32, float64, complex64 and "
+                                  "complex128 are)")
+    if isinstance(rng, np.random.Generator):
+        seed = int(rng.integers(0, 2**64, dtype=np.uint64))
+    else:
+        seed = int(rng.randint(0, 2**64, dtype=np.uint64))
+    vals = None
+    if data_sampler is not None:
+        vals = np.asarray(data_sampler(size=k)).astype(dtype, copy=False)
+        if vals.shape != (k,):
+            raise ValueError(f"{what}: the data sampler returned {vals.shape} values for {k} stored entries")
+    runtime.require_cuda(what)
+    ptr, idx, data, _ = _ops.random_csr((m, n), k, seed, _index_dtype(max(m, n)), _indptr_dtype(k), dtype,
+                                        None if vals is None else to_device(vals))
+    A = csr_array._from_parts(ptr, idx, data, (m, n))
+    if format == "csr":
+        return A
+    if format == "coo":
+        return A.tocoo()
+    if format == "dia":
+        return A.todia()
+    # csc: b2s_csr_transpose, which takes real values only; complex values follow their entries' positions, moved as
+    # float64 bit patterns (denormals).  This relies on the transpose moving values without arithmetic, as
+    # include/b200sparse.h states; the complex CSC test of tests/test_gpu_random.py fails if it ever flushes them.
+    cplx = dtype.kind == "c"
+    moved = torch.arange(k, dtype=torch.int64, device=data.device).view(torch.float64) if cplx else data
+    t_ptr, t_idx, t_val = _ops.csr_transpose(ptr, idx, moved, (m, n))
+    t_data = data[t_val.view(torch.int64)] if cplx else t_val
+    return csc_array._wrap(csr_array._from_parts(t_ptr, t_idx, t_data, (n, m)))
+
+
+@_scipy_rng(position=5)
+def random(m, n, density=0.01, format="coo", dtype=None, rng=None, data_rvs=None, *, random_state=None):
+    """A random m x n sparse matrix with exactly k = int(round(density * m * n)) stored entries at a uniform random
+    k-subset of the positions, scipy.sparse.random's signature, sampled on the device.
+
+    The values are uniform on [0, 1) (complex dtypes: real and imaginary parts each), or `data_rvs(k)`, called once
+    and cast to `dtype`, in canonical order.  float32, float64 (the default), complex64 and complex128.  `rng` and
+    `random_state` are resolved as scipy resolves them, and exactly one 64-bit seed is drawn from the result; everything
+    after that runs on the device, so one seed gives bit-identical arrays on every run and in every format ("coo", the
+    default, in row-major order, "csr", "csc", "dia").  It is not the matrix scipy draws for that seed.  The reference's
+    positional order (..., dtype, random_state, data_rvs) works unchanged."""
+    return _random((m, n), density, format, dtype, rng, None if data_rvs is None else (lambda size: data_rvs(size)),
+                   "random")
+
+
+@_scipy_rng(position=5)
+def rand(m, n, density=0.01, format="coo", dtype=None, rng=None, *, random_state=None):
+    """`random` with uniform [0, 1) values, scipy.sparse.rand's signature."""
+    return _random((m, n), density, format, dtype, rng, None, "rand")
+
+
+@_scipy_rng()
+def random_array(shape, *, density=0.01, format="coo", dtype=None, rng=None, data_sampler=None, random_state=None):
+    """`random` with scipy.sparse.random_array's signature: a 2-D `shape`, and `data_sampler(size=k)` for the values."""
+    return _random(tuple(shape), density, format, dtype, rng, data_sampler, "random_array")

@@ -22,6 +22,9 @@ from legate.sparse_b200 import (  # noqa: F401
     kron,
     kronsum,
     linalg,
+    rand,
+    random,
+    random_array,
     runtime,
     spdiags,
     vstack,
